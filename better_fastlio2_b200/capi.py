@@ -62,6 +62,16 @@ class Profile(C.Structure):
                 ("knn_head_candidates", C.c_longlong), ("knn_chain_nodes", C.c_longlong), ("knn_chain_max", C.c_longlong)]
 
 
+class PreprocessConfig(C.Structure):
+    _fields_ = [("lidar_type", C.c_int), ("n_scans", C.c_int), ("scan_rate", C.c_int), ("point_filter_num", C.c_int),
+                ("time_unit", C.c_int), ("blind", C.c_double)]
+
+
+class RawLayout(C.Structure):
+    _fields_ = [("stride", C.c_int), ("off_x", C.c_int), ("off_y", C.c_int), ("off_z", C.c_int), ("off_intensity", C.c_int),
+                ("off_time", C.c_int), ("off_ring", C.c_int), ("off_tag", C.c_int), ("off_line", C.c_int)]
+
+
 K_CLASSES = ["transform", "knn", "residual", "reduce", "classify", "insert", "delete"]
 
 _lib = None
@@ -81,6 +91,7 @@ EXPORTS = [
     "flb_frontend_points_to_world", "flb_voxel_grid_filter", "flb_map_reconstruct_keyframes",
     "flb_map_build_pt", "flb_map_reconstruct_pt", "flb_map_add_points_pt", "flb_map_nearest_search_xyzi",
     "flb_map_box_search_xyzi", "flb_map_radius_search_xyzi", "flb_map_flatten_xyzi", "flb_scan_upload_pt",
+    "flb_frontend_preprocess",
 ]
 
 
@@ -155,6 +166,8 @@ def lib():
         L.flb_frontend_download_down.argtypes = [vp, fp, fp, C.c_int, ip]
         L.flb_frontend_points_to_world.argtypes = [vp, C.c_int, dp, fp, C.c_int, ip]
         L.flb_voxel_grid_filter.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, fp, C.c_int, ip]
+        L.flb_frontend_preprocess.argtypes = [vp, C.POINTER(PreprocessConfig), C.POINTER(RawLayout), vp, C.c_int, ip,
+                                              C.POINTER(C.c_float)]
         L.flb_map_reconstruct_keyframes.argtypes = [vp, C.POINTER(vp), ip, C.c_int, C.c_int, C.c_int, fp, C.c_float, fp,
                                                     C.c_int, ip]
         _lib = L
@@ -542,6 +555,18 @@ class FrontEnd:
         self.session.n = cnt.value
         return cnt.value
 
+    def preprocess(self, records, cfg, layout=None):
+        """Preprocess::process on the device: driver records (numpy structured array in message order) -> the front
+        end's raw scan.  cfg: PreprocessConfig or preprocess_config() kwargs; layout: RawLayout, or raw_layout() name
+        overrides (default: fields found by name).  Returns (pl_surf size, last point's curvature)."""
+        rec, c, lay = _preprocess_args(records, cfg, layout)
+        self.n_raw = 0   # a failed call leaves an empty scan
+        n, last = C.c_int(0), C.c_float(0)
+        _chk(lib().flb_frontend_preprocess(self.h, C.byref(c), C.byref(lay), _p(rec) if len(rec) else None, len(rec), C.byref(n),
+                                           C.byref(last)))
+        self.n_raw = n.value
+        return n.value, np.float32(last.value)
+
     def download_undistorted(self):
         n = self.n_raw
         xyzi = np.empty((max(n, 1), 4), np.float32)
@@ -566,6 +591,40 @@ class FrontEnd:
         out = np.empty((self.cap, 4), np.float32)
         _chk(lib().flb_frontend_points_to_world(self.h, int(which), _p(st), _p(out), self.cap, C.byref(cnt)))
         return out[:cnt.value].copy()
+
+
+# Preprocess parameters (preprocess.h:8-14, laserMapping.cpp:2034-2041)
+LIVOX, VELO16, OUST64 = 1, 2, 3
+SEC, MS, US, NS = 0, 1, 2, 3
+# record field -> names matched in a structured dtype, first match wins (pcl::fromROSMsg matches fields by name)
+_FIELD_NAMES = {"x": ("x",), "y": ("y",), "z": ("z",), "intensity": ("intensity", "reflectivity"),
+                "time": ("time", "t", "offset_time"), "ring": ("ring",), "tag": ("tag",), "line": ("line",)}
+
+
+def preprocess_config(lidar_type, n_scans=16, scan_rate=10, point_filter_num=1, time_unit=MS, blind=0.01):
+    return PreprocessConfig(int(lidar_type), int(n_scans), int(scan_rate), int(point_filter_num), int(time_unit), float(blind))
+
+
+def raw_layout(dtype, **names):
+    """flb_raw_layout of a numpy structured dtype: offsets of the fields found by name; names= overrides a lookup
+    (a field name, or None for "absent")."""
+    dtype = np.dtype(dtype)
+    lay = RawLayout(dtype.itemsize, *([-1] * 8))
+    for key, cands in _FIELD_NAMES.items():
+        if key in names:
+            cands = () if names[key] is None else (names[key],)
+        for c in cands:
+            if dtype.names and c in dtype.names:
+                setattr(lay, "off_" + key, dtype.fields[c][1])
+                break
+    return lay
+
+
+def _preprocess_args(records, cfg, layout):
+    rec = np.ascontiguousarray(records)
+    c = cfg if isinstance(cfg, PreprocessConfig) else preprocess_config(**cfg)
+    lay = layout if isinstance(layout, RawLayout) else raw_layout(rec.dtype, **(layout or {}))
+    return rec, c, lay
 
 
 def voxel_grid_filter(tree, points48, leaf):

@@ -1767,3 +1767,4 @@ extern "C" int flb_debug_trace_read(unsigned long long* out, long long* phases, 
 
 // ------------------------------------------------------------------------------------------------ front-end rows (SURVEY.md §8f)
 #include "frontend_host.cuh"
+#include "preprocess_host.cuh"

@@ -67,6 +67,8 @@ static int vg_enqueue(flb_map* m, VgWork& w, const float4* pts, const float* cur
 }
 
 // ------------------------------------------------------------------------------------------------ front end object
+struct PpWork;                          // preprocess scratch (preprocess_host.cuh)
+static void pp_release(PpWork* w);
 struct flb_frontend {
   flb_session* ses = nullptr;
   int cap = 0;
@@ -82,6 +84,7 @@ struct flb_frontend {
   double *d_poses = nullptr, *h_poses = nullptr;
   cudaEvent_t ev_poses = nullptr;
   VgWork vg;
+  PpWork* pp = nullptr;
   bool holds_ref = false;
 };
 
@@ -128,12 +131,27 @@ extern "C" void flb_frontend_destroy(flb_frontend* f) {
   if (f->ev_poses) Q(cudaEventDestroy(f->ev_poses));
   const bool counted = f->holds_ref;
   vg_release(f->vg);
+  pp_release(f->pp);
   delete f;
   if (m && counted) map_release(m);
 }
 
 static inline const float4* fe_cloud(const flb_frontend* f) { return f->sorted ? f->pts_t : f->pts; }
 static inline const float* fe_curv(const flb_frontend* f) { return f->sorted ? f->curv_t : f->curv; }
+
+// copy n host records of `stride` bytes into the front end's raw staging buffer (on the session stream)
+static int fe_stage_raw(flb_frontend* f, flb_map* m, const void* src, int n, int stride) {
+  const size_t bytes = (size_t)n * stride;
+  if (bytes > f->raw_cap) {
+    if (f->raw) cudaFree(f->raw);
+    f->raw = nullptr; f->raw_cap = 0;
+    const size_t cap = std::max(bytes, (size_t)f->cap * (size_t)stride);   // sized once for the capacity: scans vary in size
+    CU(cudaMalloc((void**)&f->raw, cap));
+    f->raw_cap = cap;
+  }
+  CU(cudaMemcpyAsync(f->raw, src, bytes, cudaMemcpyHostToDevice, m->stream));
+  return 0;
+}
 
 extern "C" int flb_frontend_upload(flb_frontend* f, const void* pts, int n, int stride, int off_intensity, int off_curvature) {
   if (!f) return set_err("null front end");
@@ -147,15 +165,7 @@ extern "C" int flb_frontend_upload(flb_frontend* f, const void* pts, int n, int 
   f->sorted = false;
   f->n_down = -1;
   if (n == 0) return 0;
-  const size_t bytes = (size_t)n * stride;
-  if (bytes > f->raw_cap) {
-    if (f->raw) cudaFree(f->raw);
-    f->raw = nullptr; f->raw_cap = 0;
-    const size_t cap = std::max(bytes, (size_t)f->cap * (size_t)stride);   // sized once for the capacity: scans vary in size
-    CU(cudaMalloc((void**)&f->raw, cap));
-    f->raw_cap = cap;
-  }
-  CU(cudaMemcpyAsync(f->raw, pts, bytes, cudaMemcpyHostToDevice, m->stream));
+  if (fe_stage_raw(f, m, pts, n, stride)) return 1;
   k_pack_xyzic<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(f->raw, stride, off_intensity, off_curvature, f->pts, f->curv, n);
   m->launches++;
   CU(cudaGetLastError());

@@ -310,3 +310,99 @@ def raw_scan_with_times(body_xyz, rng, scan_time_ms=100.0, shuffle=True):
     inten = rng.uniform(0, 255, n).astype(np.float32)
     order = rng.permutation(n) if shuffle else np.arange(n)
     return body_xyz[order].astype(np.float32), inten[order], cur[order].astype(np.float32)
+
+
+# ------------------------------------------------------------------------------------------------ driver records
+# Message layouts of the three preprocessed sensor families (little endian, as on the wire):
+#   Velodyne PointCloud2 of velodyne_pointcloud: x y z intensity f32, ring u16, time f32 (s) packed, point_step 22
+#   Ouster PointCloud2 of ouster_ros (preprocess.h:109-128): x y z (+pad) intensity t(ns) reflectivity ring ambient range
+#   Livox CustomMsg CustomPoint: offset_time u32 (ns), x y z f32, reflectivity tag line u8 (20 bytes)
+VELO_DTYPE = np.dtype({"names": ["x", "y", "z", "intensity", "ring", "time"],
+                       "formats": ["<f4", "<f4", "<f4", "<f4", "<u2", "<f4"], "offsets": [0, 4, 8, 12, 16, 18], "itemsize": 22})
+VELO_DTYPE_NO_TIME = np.dtype({"names": ["x", "y", "z", "intensity", "ring"],
+                               "formats": ["<f4", "<f4", "<f4", "<f4", "<u2"], "offsets": [0, 4, 8, 12, 16], "itemsize": 18})
+OUSTER_DTYPE = np.dtype({"names": ["x", "y", "z", "intensity", "t", "reflectivity", "ring", "ambient", "range"],
+                         "formats": ["<f4", "<f4", "<f4", "<f4", "<u4", "<u2", "u1", "<u2", "<u4"],
+                         "offsets": [0, 4, 8, 16, 20, 24, 26, 28, 32], "itemsize": 48})
+LIVOX_DTYPE = np.dtype({"names": ["offset_time", "x", "y", "z", "reflectivity", "tag", "line"],
+                        "formats": ["<u4", "<f4", "<f4", "<f4", "u1", "u1", "u1"], "offsets": [0, 4, 8, 12, 16, 17, 18],
+                        "itemsize": 20})
+DRIVER_MODELS = {"vlp16": "velodyne", "hdl64": "velodyne", "os64": "ouster", "hap": "livox"}
+
+
+def driver_records(model, world, state_true, rng, with_time=True, scan_time=0.1, max_range=100.0, blind_frac=0.01,
+                   nan_frac=0.001, n_lines=4):
+    """One sweep of driver records in firing order from the same ray-cast world as scan_from_pose.
+
+    Spinning sensors (vlp16, hdl64 -> Velodyne layout; os64 -> Ouster layout) fire column by column, azimuth decreasing
+    (clockwise) from a random start, one extra column past 360 deg so every ring's time wraps; Velodyne rays without a
+    return are absent from the message, Ouster ones are zero points.  with_time=False drops the Velodyne `time` field (the
+    preprocessing then synthesises it from the azimuth).  Livox (hap) rays come in time order with line = ray % n_lines;
+    no-return rays are zero points, and the message carries second returns (tag 0x20 / 0x30), records with
+    line >= n_lines and exact repeats of the previous point.  A blind_frac share of returns sits within 0.2-1.5 m
+    (vehicle body) and a nan_frac share is NaN."""
+    kind = DRIVER_MODELS[model]
+    R = quat_to_mat(state_true[3:7])
+    Rli = quat_to_mat(state_true[7:11])
+    o = state_true[0:3] + R @ state_true[11:14]
+    if kind == "livox":
+        dirs = lidar_dirs(model, rng)
+        n = len(dirs)
+        ring = np.arange(n) % n_lines
+        frac = np.arange(n) / n
+    else:
+        el = {"vlp16": np.linspace(-15, 15, 16), "hdl64": np.linspace(2.0, -24.8, 64), "os64": np.linspace(16.6, -16.6, 64)}[model]
+        n_az = {"vlp16": 1800, "hdl64": 1875, "os64": 1024}[model]
+        az0 = rng.uniform(0, 360)
+        az = az0 - np.arange(n_az + 1) * (360.0 / n_az)           # clockwise, one column of overlap
+        A, E = np.meshgrid(np.deg2rad(az), np.deg2rad(el), indexing="ij")   # column-major firing order
+        dirs = np.stack([(np.cos(E) * np.cos(A)).ravel(), (np.cos(E) * np.sin(A)).ravel(), np.sin(E).ravel()], 1)
+        ring = np.tile(np.arange(len(el)), n_az + 1)
+        frac = np.repeat(np.arange(n_az + 1) / n_az, len(el))
+    t = raycast(world, o, dirs @ (R @ Rli).T, max_range, 0.5)
+    hit = np.isfinite(t)
+    t = np.where(hit, t + rng.normal(0, 0.01, len(t)), 0.0)
+    close = rng.random(len(t)) < blind_frac
+    t[close] = rng.uniform(0.2, 1.5, close.sum())
+    hit |= close
+    xyz = (dirs * t[:, None]).astype(np.float32)
+    xyz[rng.random(len(t)) < nan_frac] = np.nan
+    inten = rng.uniform(0, 255, len(t)).astype(np.float32)
+    if kind == "velodyne":
+        keep = hit
+        rec = np.zeros(int(keep.sum()), VELO_DTYPE if with_time else VELO_DTYPE_NO_TIME)
+        for k, c in enumerate("xyz"):
+            rec[c] = xyz[keep, k]
+        rec["intensity"] = inten[keep]
+        rec["ring"] = ring[keep]
+        if with_time:
+            rec["time"] = (frac[keep] * scan_time).astype(np.float32)
+        return rec
+    if kind == "ouster":
+        rec = np.zeros(len(t), OUSTER_DTYPE)
+        for k, c in enumerate("xyz"):
+            rec[c] = xyz[:, k]
+        rec["intensity"] = inten
+        rec["t"] = np.round(frac * scan_time * 1e9).astype(np.uint32)
+        rec["reflectivity"] = rng.integers(0, 1 << 16, len(t))
+        rec["ring"] = ring
+        rec["range"] = np.round(t * 1000).astype(np.uint32)
+        return rec
+    # Livox: first returns in time order, then second returns / foreign lines / repeats spliced in
+    rec = np.zeros(len(t), LIVOX_DTYPE)
+    for k, c in enumerate("xyz"):
+        rec[c] = xyz[:, k]
+    rec["offset_time"] = np.round(frac * scan_time * 1e9).astype(np.uint32)
+    rec["reflectivity"] = inten.astype(np.uint8)
+    rec["line"] = ring
+    rec["tag"] = rng.choice([0x00, 0x10], len(t), p=[0.9, 0.1])
+    extra = rng.choice(len(t), max(1, len(t) // 50), replace=False)
+    dup = rec[extra].copy()
+    kind_x = rng.integers(0, 3, len(dup))
+    dup["tag"] = np.where(kind_x == 0, 0x20, np.where(kind_x == 1, 0x30, dup["tag"]))
+    dup["line"] = np.where(kind_x == 2, n_lines + rng.integers(0, 3, len(dup)), dup["line"])
+    rep = rng.choice(len(t), max(1, len(t) // 200), replace=False)
+    rep_rec = rec[rep].copy()
+    ins = np.concatenate([extra + 1, rep + 1])
+    order = np.argsort(ins, kind="stable")
+    return np.insert(rec, ins[order], np.concatenate([dup, rep_rec])[order])

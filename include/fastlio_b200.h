@@ -285,6 +285,44 @@ int flb_frontend_download_down(flb_frontend* f, float* out_xyzi, float* out_curv
  * feats_down_body (which = 0, dense_pub_en false) or feats_undistort (which = 1) with the posterior state. */
 int flb_frontend_points_to_world(flb_frontend* f, int which, const double* state26, float* out_xyzi, int cap, int* n);
 
+/* Preprocess::process (src/preprocess.cpp) with feature extraction off (feature_extract_enable, laserMapping.cpp:2040):
+ * driver records -> the PointType cloud that becomes meas.lidar, on the device.  Parameters as read at
+ * laserMapping.cpp:2034-2041 (preprocess.h:8-14 for the enums):
+ *   lidar_type 1 LIVOX   CustomMsg     livox_handler, feature-off branch (preprocess.cpp:178-204)
+ *              2 VELO16  PointCloud2   velodyne_handler (:302-340, :417-473); per-point time synthesised from the
+ *                                      azimuth, ring by ring, when the last record's time is not > 0
+ *              3 OUST64  PointCloud2   oust64_handler, feature-off branch (:271-297)
+ *   time_unit  0 SEC, 1 MS, 2 US, 3 NS (time_unit_scale 1e3f, 1, 1e-3f, 1e-6f; preprocess.cpp:65-82)
+ * Record fields (byte offsets inside one record of `stride` bytes, -1 = absent, read as 0 like pcl::fromROSMsg does for
+ * a field with no match; x, y, z are required).  Field types are fixed per sensor:
+ *   LIVOX   off_time = offset_time u32 (ns), off_intensity = reflectivity u8, off_tag u8, off_line u8, x y z f32
+ *   VELO16  x y z intensity f32, off_time = time f32, off_ring = ring u16            (preprocess.h:94-107)
+ *   OUST64  x y z intensity f32, off_time = t u32                                      (preprocess.h:109-128)
+ * Offsets need no alignment (packed PointCloud2 layouts such as point_step 22 are read as they are). */
+typedef struct {
+  int lidar_type;        /* 1 LIVOX, 2 VELO16, 3 OUST64 */
+  int n_scans;           /* preprocess/scan_line */
+  int scan_rate;         /* preprocess/scan_rate (Hz) */
+  int point_filter_num;  /* point_filter_num, >= 1 */
+  int time_unit;         /* preprocess/timestamp_unit */
+  double blind;          /* preprocess/blind (m) */
+} flb_preprocess_config;
+
+typedef struct {
+  int stride;            /* bytes per record (PointCloud2 point_step, sizeof(CustomPoint)) */
+  int off_x, off_y, off_z, off_intensity, off_time, off_ring, off_tag, off_line;
+} flb_raw_layout;
+
+/* Decode, decimate, blind-cut and time-stamp n driver records in one upload and one synchronisation; the kept points
+ * (input order, normals zero) become the front end's current raw scan exactly as flb_frontend_upload would leave it, so
+ * flb_frontend_undistort / _voxel_filter / _download_undistorted follow unchanged.  *n_out = pl_surf.size() and
+ * *last_curvature = pl_surf.points.back().curvature (0 for an empty result): what sync_packages needs for
+ * lidar_end_time (laserMapping.cpp:1374-1405).  Either output pointer may be NULL.  Arguments are validated before any
+ * device work; a Velodyne ring >= n_scans (undefined behaviour in the reference) fails the call and leaves an empty
+ * scan. */
+int flb_frontend_preprocess(flb_frontend* f, const flb_preprocess_config* cfg, const flb_raw_layout* layout, const void* records,
+                            int n, int* n_out, float* last_curvature);
+
 /* Stand-alone pcl::VoxelGrid centroid filter on a host cloud (the reference's other VoxelGrid call sites, e.g.
  * laserMapping.cpp:640-643, :1780-1789), run on the map's device/stream.  out_xyzi = x,y,z,intensity per point. */
 int flb_voxel_grid_filter(flb_map* m, const void* pts, int n, int stride_bytes, int off_intensity, float leaf_size,
