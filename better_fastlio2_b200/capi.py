@@ -92,6 +92,9 @@ EXPORTS = [
     "flb_map_build_pt", "flb_map_reconstruct_pt", "flb_map_add_points_pt", "flb_map_nearest_search_xyzi",
     "flb_map_box_search_xyzi", "flb_map_radius_search_xyzi", "flb_map_flatten_xyzi", "flb_scan_upload_pt",
     "flb_frontend_preprocess",
+    "flb_keyframes_create", "flb_keyframes_destroy", "flb_keyframes_append_frontend", "flb_keyframes_append",
+    "flb_keyframes_download", "flb_keyframes_info", "flb_keyframes_size", "flb_map_reconstruct_from_keyframes",
+    "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
 ]
 
 
@@ -170,6 +173,18 @@ def lib():
                                               C.POINTER(C.c_float)]
         L.flb_map_reconstruct_keyframes.argtypes = [vp, C.POINTER(vp), ip, C.c_int, C.c_int, C.c_int, fp, C.c_float, fp,
                                                     C.c_int, ip]
+        llp = C.POINTER(C.c_longlong)
+        L.flb_keyframes_create.argtypes = [vp, C.c_longlong, C.c_int, C.POINTER(vp)]
+        L.flb_keyframes_destroy.argtypes = [vp]
+        L.flb_keyframes_destroy.restype = None
+        L.flb_keyframes_append_frontend.argtypes = [vp, vp, ip]
+        L.flb_keyframes_append.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, ip]
+        L.flb_keyframes_download.argtypes = [vp, C.c_int, fp, fp, C.c_int, ip]
+        L.flb_keyframes_info.argtypes = [vp, ip, llp, llp, llp]
+        L.flb_map_release_keyframe_scratch.argtypes = [vp]
+        L.flb_keyframes_size.argtypes = [vp, C.c_int]
+        L.flb_map_reconstruct_from_keyframes.argtypes = [vp, vp, vp, C.c_int, fp, C.c_float, fp, C.c_int, ip]
+        L.flb_keyframes_assemble.argtypes = [vp, vp, C.c_int, C.c_int, fp, C.c_float, fp, fp, C.c_int, ip]
         _lib = L
     return _lib
 
@@ -649,6 +664,106 @@ def reconstruct_keyframes(tree, clouds48, poses6, leaf):
     _chk(lib().flb_map_reconstruct_keyframes(tree.h, ptrs, sizes, k, POINT_STRIDE, OFF_INTENSITY, _p(p6), float(leaf), _p(out),
                                              len(out), C.byref(n)))
     return out[:n.value].copy()
+
+
+KF_POSE6, KF_AFFINE = 0, 1   # FLB_KF_POSE6 / FLB_KF_AFFINE
+
+
+class KeyFrameStore:
+    """surfCloudKeyFrames on the device (laserMapping.cpp:756-758): body-frame key-frame clouds, x,y,z,intensity +
+    curvature, in a fixed-capacity append-only arena on the map's device; every reader takes the poses at call time."""
+
+    def __init__(self, tree, max_points, max_keyframes):
+        self.tree = tree
+        self.h = C.c_void_p()
+        _chk(lib().flb_keyframes_create(tree.h, int(max_points), int(max_keyframes), C.byref(self.h)))
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().flb_keyframes_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def append_frontend(self, fe):
+        """The front end's current feats_undistort becomes the next key frame (device to device). Returns its id."""
+        k = C.c_int(-1)
+        _chk(lib().flb_keyframes_append_frontend(self.h, fe.h, C.byref(k)))
+        return k.value
+
+    def append(self, points48):
+        """(n,12) float32 PointType records (see pack_pointtype). Returns the new key frame's id."""
+        b = np.ascontiguousarray(points48, np.float32).reshape(-1, 12)
+        k = C.c_int(-1)
+        _chk(lib().flb_keyframes_append(self.h, _p(b) if len(b) else None, len(b), POINT_STRIDE, OFF_INTENSITY, OFF_CURVATURE,
+                                        C.byref(k)))
+        return k.value
+
+    def size(self, k):
+        v = lib().flb_keyframes_size(self.h, int(k))
+        if v < 0:
+            raise FlbError(lib().flb_last_error().decode())
+        return v
+
+    def info(self):
+        nk, npts, nb, ns = C.c_int(0), C.c_longlong(0), C.c_longlong(0), C.c_longlong(0)
+        _chk(lib().flb_keyframes_info(self.h, C.byref(nk), C.byref(npts), C.byref(nb), C.byref(ns)))
+        return {"n_keyframes": nk.value, "n_points": npts.value, "device_bytes": nb.value, "map_scratch_bytes": ns.value}
+
+    def release_scratch(self):
+        """Free the readers' scratch the map keeps (e.g. after a save map); the next reader allocates again."""
+        _chk(lib().flb_map_release_keyframe_scratch(self.tree.h))
+
+    def download(self, k):
+        """Key frame k as stored: ((n,4) x,y,z,intensity, (n,) curvature)."""
+        n = self.size(k)
+        xyzi = np.empty((max(n, 1), 4), np.float32)
+        cur = np.empty(max(n, 1), np.float32)
+        cnt = C.c_int(0)
+        _chk(lib().flb_keyframes_download(self.h, int(k), _p(xyzi), _p(cur), n, C.byref(cnt)))
+        return xyzi[:n].copy(), cur[:n].copy()
+
+    def _selection_size(self, ids):
+        return sum(self.size(int(i)) for i in ids) if len(ids) else 0
+
+    def reconstruct(self, ids, poses6, leaf, cap=None):
+        """recontructIKdTree from the store: transform ids[j] by poses6[j], concatenate, VoxelGrid(leaf), rebuild the map.
+        Returns featsFromMap ((m,4) x,y,z,intensity)."""
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        p6 = np.ascontiguousarray(poses6, np.float32).reshape(-1, 6)
+        if len(p6) != len(ids):
+            raise ValueError("one pose per selected key frame")
+        cap = self._selection_size(ids) if cap is None else int(cap)
+        out = np.empty((max(cap, 1), 4), np.float32)
+        n = C.c_int(0)
+        _chk(lib().flb_map_reconstruct_from_keyframes(self.tree.h, self.h, _p(ids) if len(ids) else None, len(ids),
+                                                      _p(p6) if len(ids) else None, float(leaf), _p(out), cap, C.byref(n)))
+        return out[:min(n.value, cap)].copy()
+
+    def assemble(self, ids, poses6=None, affines=None, leaf=0.0, cap=None, return_size=False):
+        """Concatenate ids in order, each transformed by its pose6 (x,y,z,roll,pitch,yaw) or its row-major 3x4 affine;
+        leaf > 0 filters with pcl::VoxelGrid (curvature carried).  Returns ((m,4) x,y,z,intensity, (m,) curvature)
+        [, full size when return_size]."""
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        if (poses6 is None) == (affines is None):
+            raise ValueError("pass exactly one of poses6 / affines")
+        kind = KF_POSE6 if poses6 is not None else KF_AFFINE
+        tr = np.ascontiguousarray(poses6 if poses6 is not None else affines, np.float32).reshape(-1)
+        if len(tr) != len(ids) * (6 if kind == KF_POSE6 else 12):
+            raise ValueError("one transform per selected key frame")
+        cap = self._selection_size(ids) if cap is None else int(cap)
+        xyzi = np.empty((max(cap, 1), 4), np.float32)
+        cur = np.empty(max(cap, 1), np.float32)
+        n = C.c_int(0)
+        _chk(lib().flb_keyframes_assemble(self.h, _p(ids) if len(ids) else None, len(ids), kind, _p(tr) if len(ids) else None,
+                                          float(leaf), _p(xyzi), _p(cur), cap, C.byref(n)))
+        m = min(n.value, cap)
+        res = (xyzi[:m].copy(), cur[:m].copy())
+        return res + (n.value,) if return_size else res
 
 
 def make_fov(cube_len=200.0, det_range=100.0):

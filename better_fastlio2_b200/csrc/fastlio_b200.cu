@@ -121,7 +121,8 @@ struct flb_map {
   bool scratch_clean = false;    // the downsample scratch hash was already cleared off the critical path (scan graph)
   unsigned char* kf_raw = nullptr;   // flb_map_reconstruct_keyframes scratch (grow-only)
   float4 *kf_in = nullptr, *kf_out = nullptr;
-  size_t kf_raw_cap = 0, kf_pts_cap = 0;
+  size_t kf_raw_cap = 0, kf_in_cap = 0, kf_out_cap = 0;   // bytes
+  struct KfWork* kfw = nullptr;      // the rest of the key-frame readers' scratch (keyframe_host.cuh, grow-only)
   int gen = 0;                   // bumped whenever a buffer or parameter baked into a captured scan graph changes (scratch hash,
                                  // work list, voxel size): sessions re-capture their graphs on a mismatch
   bool warned_range = false;
@@ -259,6 +260,7 @@ extern "C" int flb_map_create(const flb_map_config* cfg, flb_map** out) {
 }
 
 static void map_release(flb_map* m);
+static void kfw_release(KfWork* w);
 extern "C" void flb_map_destroy(flb_map* m) {
   if (!m) return;
   map_release(m);  // sessions created on this map keep it alive until they are destroyed too
@@ -272,6 +274,7 @@ static void map_release(flb_map* m) {
                   m->d_misc, m->stage, m->raw, m->skeys, m->sbest, m->dparams, m->outbuf, m->d_phase, m->worklist, m->kf_raw, m->kf_in, m->kf_out};
   for (void* p : ptrs) if (p) Q(cudaFree(p));
   if (m->h_counters) Q(cudaFreeHost(m->h_counters));
+  kfw_release(m->kfw);
   for (auto& r : m->prof_pool) { Q(cudaEventDestroy(r.a)); Q(cudaEventDestroy(r.b)); }
   if (m->stream) Q(cudaStreamDestroy(m->stream));
   delete m;
@@ -1768,3 +1771,4 @@ extern "C" int flb_debug_trace_read(unsigned long long* out, long long* phases, 
 // ------------------------------------------------------------------------------------------------ front-end rows (SURVEY.md §8f)
 #include "frontend_host.cuh"
 #include "preprocess_host.cuh"
+#include "keyframe_host.cuh"

@@ -336,6 +336,59 @@ int flb_map_reconstruct_keyframes(flb_map* m, const void* const* clouds, const i
                                   int off_intensity, const float* poses6, float leaf_size, float* out_xyzi, int cap,
                                   int* n_points);
 
+/* ------------------------------------------------------------------------------------------------ key-frame store
+ * surfCloudKeyFrames (laserMapping.cpp:756-758) kept on the device: each key frame is the whole undistorted scan
+ * (feats_undistort) in its own body frame, stored as x,y,z,intensity + curvature (20 bytes per point) in a fixed-capacity,
+ * append-only arena sized at creation.  Poses are not stored (iSAM2 rewrites them, correctPoses :780-795): every reader
+ * takes them at call time.  A store is created on a map, uses its device and stream and keeps it alive until destroyed.
+ * The library takes no lock: calls on a store are serialised by the caller with every other call on that map, from all
+ * threads (a loop-closure thread and the main loop hold one common mutex around their calls, INTEGRATION.md §3, §5).
+ * Every call validates all its arguments before any device work; a failed call leaves the store unchanged. */
+typedef struct flb_keyframes flb_keyframes;
+#define FLB_KF_POSE6 0  /* transforms = n_ids x {x, y, z, roll, pitch, yaw}: pcl::getTransformation, as transformPointCloud
+                           with a PointTypePose (common_lib.h:711-734) */
+#define FLB_KF_AFFINE 1 /* transforms = n_ids x row-major 3x4 float affine (e.g. keyTrans.inverse() * keyNearTrans,
+                           laserMapping.cpp:873-875); an affine equal to the identity copies the stored records verbatim,
+                           curvature included (*nearKeyframes += *surfCloudKeyFrames[key], :869).  The test is on the
+                           values: any entry whose affine is exactly the identity is copied, not computed */
+
+int flb_keyframes_create(flb_map* m, long long max_points, int max_keyframes, flb_keyframes** out);
+void flb_keyframes_destroy(flb_keyframes* kf);
+/* pcl::copyPointCloud(*feats_undistort, *thisSurfKeyFrame); surfCloudKeyFrames.push_back(...)  (laserMapping.cpp:756-758):
+ * appends the front end's current scan (time-sorted and compensated after flb_frontend_undistort, else in upload order) as
+ * the next key frame, device to device on the map stream with no synchronisation.  *index = the new key frame's id.
+ * Fails when the front end's session is on another map or either capacity would be exceeded. */
+int flb_keyframes_append_frontend(flb_keyframes* kf, flb_frontend* fe, int* index);
+/* The same from n host records (restoring a session, tests): offsets as flb_frontend_upload. */
+int flb_keyframes_append(flb_keyframes* kf, const void* pts, int n, int stride_bytes, int off_intensity, int off_curvature,
+                         int* index);
+/* Key frame `id` as stored: x,y,z,intensity per point and curvature (either pointer may be NULL); at most cap points are
+ * written, *n = its size (copyPointCloud(*surfCloudKeyFrames[i]) of the per-key-frame saver, laserMapping.cpp:2504). */
+int flb_keyframes_download(flb_keyframes* kf, int id, float* out_xyzi, float* out_curvature, int cap, int* n);
+/* Number of key frames, stored points and device bytes held by the store, and the device bytes of the readers' scratch
+ * its map currently holds (any pointer may be NULL).  No device work. */
+int flb_keyframes_info(const flb_keyframes* kf, int* n_keyframes, long long* n_points, long long* device_bytes,
+                       long long* map_scratch_bytes);
+/* Size of key frame `id`, or -1 (with flb_last_error) when it does not exist. */
+int flb_keyframes_size(const flb_keyframes* kf, int id);
+/* flb_map_reconstruct_keyframes with the clouds taken from the store: for j < n_ids, subMap += transformPointCloud(
+ * key frame ids[j], poses6[j]) in that order, VoxelGrid(leaf), ikdtree.reconstruct(result); featsFromMap out.  The store
+ * must have been created on m.  The selection (radius search over the key poses, :621-635) stays with the caller. */
+int flb_map_reconstruct_from_keyframes(flb_map* m, const flb_keyframes* kf, const int* ids, int n_ids, const float* poses6,
+                                       float leaf_size, float* out_xyzi, int cap, int* n_points);
+/* Map assembly from the store, ids in order, each key frame with its own transform (transform_kind FLB_KF_POSE6 or
+ * FLB_KF_AFFINE); transformed points get curvature 0 as transformPointCloud writes them.  leaf_size > 0: pcl::VoxelGrid
+ * centroid filter with curvature carried (publishGlobalMap :1866-1869, SurfMap.pcd / filterGlobalMap.pcd :1780-1789;
+ * PCL's int32 overflow guard returns the assembled cloud unchanged); leaf_size == 0: the dense concatenation
+ * (GlobalMap.pcd :1796, loop sub-maps :856-883).  At most cap points are written, *n_out = the full size (size the buffer
+ * from flb_keyframes_info / flb_keyframes_size beforehand). */
+int flb_keyframes_assemble(flb_keyframes* kf, const int* ids, int n_ids, int transform_kind, const float* transforms,
+                           float leaf_size, float* out_xyzi, float* out_curvature, int cap, int* n_out);
+/* The readers above keep their scratch with the map, grown to the largest selection so far and only for what a call
+ * uses (a dense assembly needs no filter buffers): a save map of the whole run can leave gigabytes behind.  This frees
+ * all of it (waits for the map's stream); the next reader allocates again. */
+int flb_map_release_keyframe_scratch(flb_map* m);
+
 /* Stream access for callers that overlap work (returns a cudaStream_t as void*). */
 void* flb_session_stream(flb_session* s);
 int flb_session_sync(flb_session* s);

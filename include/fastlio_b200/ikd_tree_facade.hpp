@@ -159,6 +159,8 @@ class KD_TREE {
   }
 
   flb_map* handle() { ensure(); return map_; }  // for flb_session_create
+  // Root_Node after the map was rebuilt through another C-ABI call on handle() (flb::KeyFrameStore::reconstruct)
+  void refresh_root() { sync_root(); }
   const std::string& last_error() const { return err_; }
 
   PointVector PCL_Storage;           // ikd_Tree.h:247

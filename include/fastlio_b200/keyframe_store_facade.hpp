@@ -1,0 +1,176 @@
+// keyframe_store_facade.hpp — surfCloudKeyFrames (src/laserMapping.cpp:756-758) kept on the GPU, with the reader shapes
+// laserMapping.cpp uses, so that no key-frame cloud has to live in host RAM:
+//
+//   flb::KeyFrameStore keyframes;  keyframes.attach(ikdtree.handle(), 40000000LL, 4000);   // next to `flb::LioGpu gpu;`
+//   // saveKeyFramesAndFactor, instead of :756-758 (copyPointCloud(*feats_undistort) + push_back):
+//   keyframes.push_back(fe);                                             // fe: the flb::ScanFrontEnd of the scan
+//   // recontructIKdTree, instead of :636-664 (transform + VoxelGrid + ikdtree.reconstruct + featsFromMap):
+//   keyframes.reconstruct(ikdtree, ids, *cloudKeyPoses6D, leaf, featsFromMap->points);
+//   // publishGlobalMap (:1858-1869) and saveMapService (:1763-1798): poses per key frame, leaf 0 = dense
+//   keyframes.assemble(ids, *cloudKeyPoses6D, globalMapVisualizationLeafSize, *globalMapKeyFramesDS);
+//   // loopFindNearKeyframes (:856-883): one affine per key frame, the identity for keyNear == key
+//   keyframes.assemble(ids, finalTrans, 0.f, *nearKeyframes);
+//   // the per-key-frame saver at shutdown (:2501-2505):
+//   keyframes.at(i, *save_cloud);
+//
+// Poses6D is anything with points[k].{x, y, z, roll, pitch, yaw} (pcl::PointCloud<PointTypePose>); an affine is
+// anything with operator()(row, col) (Eigen::Affine3f).  Clouds come back with x, y, z, intensity and curvature set
+// and the other PointType fields zero.  Nothing here takes a lock: calls are serialised with every other call on the map
+// from all threads — the loop-closure thread and the main loop hold one common mutex around their calls (INTEGRATION.md
+// §3 "Key-frame clouds on the GPU", §5).  Errors are reported on stderr and returned as false / -1.
+#pragma once
+#include <cstdio>
+#include <type_traits>
+#include <vector>
+
+#include "../fastlio_b200.h"
+#include "ikd_tree_facade.hpp"
+#include "scan_frontend_facade.hpp"
+
+namespace flb {
+
+class KeyFrameStore {
+ public:
+  KeyFrameStore() = default;
+  KeyFrameStore(const KeyFrameStore&) = delete;
+  KeyFrameStore& operator=(const KeyFrameStore&) = delete;
+  ~KeyFrameStore() { if (kf_) flb_keyframes_destroy(kf_); }
+
+  // capacity: points over all key frames (20 device bytes each) and number of key frames
+  bool attach(flb_map* map, long long max_points, int max_keyframes) {
+    if (flb_keyframes_create(map, max_points, max_keyframes, &kf_)) { kf_ = nullptr; return ok(1, "attach"); }
+    map_ = map;
+    return true;
+  }
+  flb_keyframes* handle() { return kf_; }
+
+  int size() const {   // surfCloudKeyFrames.size()
+    int n = 0;
+    return kf_ && !flb_keyframes_info(kf_, &n, nullptr, nullptr, nullptr) ? n : 0;
+  }
+  int points(int k) const { return kf_ ? flb_keyframes_size(kf_, k) : -1; }
+  // device bytes of the readers' scratch the map keeps, and a way to free it (e.g. at the end of saveMapService)
+  long long scratch_bytes() const {
+    long long b = 0;
+    return kf_ && !flb_keyframes_info(kf_, nullptr, nullptr, nullptr, &b) ? b : 0;
+  }
+  bool release_scratch() { return map_ && ok(flb_map_release_keyframe_scratch(map_), "release_scratch"); }
+
+  // surfCloudKeyFrames.push_back(copy of feats_undistort): the front end's current scan, device to device.  Returns the
+  // key frame's id, or -1.
+  int push_back(ScanFrontEnd& fe) {
+    int id = -1;
+    return ok(flb_keyframes_append_frontend(kf_, fe.handle(), &id), "push_back") ? id : -1;
+  }
+  // the same from a host cloud (restoring a saved session)
+  template <class Cloud>
+  int push_back(const Cloud& cloud) {
+    typedef typename std::remove_reference<decltype(cloud.points[0])>::type P;
+    const int n = (int)cloud.points.size();
+    const P* p0 = n ? &cloud.points[0] : nullptr;
+    const int off_i = n ? (int)((const char*)&p0->intensity - (const char*)p0) : -1;
+    const int off_c = n ? (int)((const char*)&p0->curvature - (const char*)p0) : -1;
+    int id = -1;
+    return ok(flb_keyframes_append(kf_, p0, n, (int)sizeof(P), off_i, off_c, &id), "push_back") ? id : -1;
+  }
+
+  // recontructIKdTree (laserMapping.cpp:636-664): subMap += transformPointCloud(key frame ids[j], poses.points[ids[j]]),
+  // VoxelGrid(leaf), tree.reconstruct, featsFromMap = the filtered sub-map.
+  template <class PointT, class Poses6D, class PointVec>
+  bool reconstruct(KD_TREE<PointT>& tree, const std::vector<int>& ids, const Poses6D& poses, float leaf, PointVec& featsFromMap) {
+    const std::vector<float> p6 = poses6(ids, poses);
+    const int cap = selection_size(ids);
+    if (cap < 0) return false;
+    xyzi_.resize((size_t)cap * 4 + 4);
+    int n = 0;
+    const bool good = ok(flb_map_reconstruct_from_keyframes(tree.handle(), kf_, ids.data(), (int)ids.size(), p6.data(), leaf, xyzi_.data(),
+                                                            cap, &n), "reconstruct");
+    tree.refresh_root();
+    if (!good) return false;
+    featsFromMap.resize(n);
+    for (int i = 0; i < n; ++i) fill(featsFromMap[i], &xyzi_[4 * (size_t)i], 0.f);
+    return true;
+  }
+
+  // *out = sum over j of transformPointCloud(key frame ids[j], poses.points[ids[j]]), VoxelGrid(leaf) when leaf > 0
+  template <class Poses6D, class Cloud>
+  bool assemble(const std::vector<int>& ids, const Poses6D& poses, float leaf, Cloud& out) {
+    const std::vector<float> p6 = poses6(ids, poses);
+    return run_assemble(ids, FLB_KF_POSE6, p6, leaf, out);
+  }
+  // the same with one affine per selected key frame (T[j] for ids[j]); the identity copies the stored records
+  template <class Affine, class Alloc, class Cloud>
+  bool assemble(const std::vector<int>& ids, const std::vector<Affine, Alloc>& T, float leaf, Cloud& out) {
+    if (T.size() != ids.size()) return ok(1, "assemble: one affine per key frame");
+    std::vector<float> t(ids.size() * 12);
+    for (size_t j = 0; j < ids.size(); ++j)
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 4; ++c) t[j * 12 + r * 4 + c] = T[j](r, c);
+    return run_assemble(ids, FLB_KF_AFFINE, t, leaf, out);
+  }
+
+  // pcl::copyPointCloud(*surfCloudKeyFrames[k], out)
+  template <class Cloud>
+  bool at(int k, Cloud& out) {
+    const int cap = points(k);
+    if (cap < 0) return ok(1, "at");
+    xyzi_.resize((size_t)cap * 4 + 4);
+    curv_.resize((size_t)cap + 1);
+    int n = 0;
+    if (!ok(flb_keyframes_download(kf_, k, xyzi_.data(), curv_.data(), cap, &n), "at")) return false;
+    out.points.resize(n);
+    for (int i = 0; i < n; ++i) fill(out.points[i], &xyzi_[4 * (size_t)i], curv_[i]);
+    return true;
+  }
+
+ private:
+  template <class Poses6D>
+  static std::vector<float> poses6(const std::vector<int>& ids, const Poses6D& poses) {
+    std::vector<float> p(ids.size() * 6 + 6, 0.f);
+    for (size_t j = 0; j < ids.size(); ++j) {
+      if (ids[j] < 0 || (size_t)ids[j] >= poses.points.size()) continue;   // the store rejects the id
+      const auto& q = poses.points[ids[j]];
+      float* o = &p[j * 6];
+      o[0] = q.x; o[1] = q.y; o[2] = q.z; o[3] = q.roll; o[4] = q.pitch; o[5] = q.yaw;
+    }
+    return p;
+  }
+  int selection_size(const std::vector<int>& ids) const {
+    long long t = 0;
+    for (int k : ids) {
+      const int c = points(k);
+      if (c < 0) { ok(1, "selection"); return -1; }
+      t += c;
+    }
+    if (t > 0x7fffffffLL) { std::fprintf(stderr, "[fastlio_b200] selection of %lld points is too large\n", t); return -1; }
+    return (int)t;
+  }
+  template <class Cloud>
+  bool run_assemble(const std::vector<int>& ids, int kind, const std::vector<float>& t, float leaf, Cloud& out) {
+    const int cap = selection_size(ids);
+    if (cap < 0) return false;
+    xyzi_.resize((size_t)cap * 4 + 4);
+    curv_.resize((size_t)cap + 1);
+    int n = 0;
+    if (!ok(flb_keyframes_assemble(kf_, ids.data(), (int)ids.size(), kind, t.data(), leaf, xyzi_.data(), curv_.data(), cap, &n), "assemble"))
+      return false;
+    out.points.resize(n);
+    for (int i = 0; i < n; ++i) fill(out.points[i], &xyzi_[4 * (size_t)i], curv_[i]);
+    return true;
+  }
+  template <class P>
+  static void fill(P& p, const float* v, float curvature) {
+    p = P();
+    p.x = v[0]; p.y = v[1]; p.z = v[2]; p.intensity = v[3]; p.curvature = curvature;
+  }
+  static bool ok(int rc, const char* what) {
+    if (rc) std::fprintf(stderr, "[fastlio_b200] KeyFrameStore::%s: %s\n", what, flb_last_error());
+    return rc == 0;
+  }
+
+  flb_keyframes* kf_ = nullptr;
+  flb_map* map_ = nullptr;
+  std::vector<float> xyzi_, curv_;
+};
+
+}  // namespace flb
