@@ -95,6 +95,7 @@ EXPORTS = [
     "flb_keyframes_create", "flb_keyframes_destroy", "flb_keyframes_append_frontend", "flb_keyframes_append",
     "flb_keyframes_download", "flb_keyframes_info", "flb_keyframes_size", "flb_map_reconstruct_from_keyframes",
     "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
+    "flb_keyframes_scan_context", "flb_keyframes_scan_contexts",
 ]
 
 
@@ -185,6 +186,8 @@ def lib():
         L.flb_keyframes_size.argtypes = [vp, C.c_int]
         L.flb_map_reconstruct_from_keyframes.argtypes = [vp, vp, vp, C.c_int, fp, C.c_float, fp, C.c_int, ip]
         L.flb_keyframes_assemble.argtypes = [vp, vp, C.c_int, C.c_int, fp, C.c_float, fp, fp, C.c_int, ip]
+        L.flb_keyframes_scan_context.argtypes = [vp, vp, C.c_int, C.c_int, fp, C.c_double, dp]
+        L.flb_keyframes_scan_contexts.argtypes = [vp, vp, C.c_int, C.c_double, dp]
         _lib = L
     return _lib
 
@@ -667,6 +670,7 @@ def reconstruct_keyframes(tree, clouds48, poses6, leaf):
 
 
 KF_POSE6, KF_AFFINE = 0, 1   # FLB_KF_POSE6 / FLB_KF_AFFINE
+SC_RINGS, SC_SECTORS = 20, 60  # FLB_SC_RINGS / FLB_SC_SECTORS
 
 
 class KeyFrameStore:
@@ -749,12 +753,7 @@ class KeyFrameStore:
         leaf > 0 filters with pcl::VoxelGrid (curvature carried).  Returns ((m,4) x,y,z,intensity, (m,) curvature)
         [, full size when return_size]."""
         ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
-        if (poses6 is None) == (affines is None):
-            raise ValueError("pass exactly one of poses6 / affines")
-        kind = KF_POSE6 if poses6 is not None else KF_AFFINE
-        tr = np.ascontiguousarray(poses6 if poses6 is not None else affines, np.float32).reshape(-1)
-        if len(tr) != len(ids) * (6 if kind == KF_POSE6 else 12):
-            raise ValueError("one transform per selected key frame")
+        kind, tr = self._transforms(ids, poses6, affines)
         cap = self._selection_size(ids) if cap is None else int(cap)
         xyzi = np.empty((max(cap, 1), 4), np.float32)
         cur = np.empty(max(cap, 1), np.float32)
@@ -764,6 +763,34 @@ class KeyFrameStore:
         m = min(n.value, cap)
         res = (xyzi[:m].copy(), cur[:m].copy())
         return res + (n.value,) if return_size else res
+
+    @staticmethod
+    def _transforms(ids, poses6, affines):
+        if (poses6 is None) == (affines is None):
+            raise ValueError("pass exactly one of poses6 / affines")
+        kind = KF_POSE6 if poses6 is not None else KF_AFFINE
+        tr = np.ascontiguousarray(poses6 if poses6 is not None else affines, np.float32).reshape(-1)
+        if len(tr) != len(ids) * (6 if kind == KF_POSE6 else 12):
+            raise ValueError("one transform per selected key frame")
+        return kind, tr
+
+    def scan_context(self, ids, poses6=None, affines=None, lidar_height=1.5):
+        """SCManager::makeScancontext of the dense assembly of ids (transforms as assemble), computed on the device:
+        (20, 60) float64, row-major (ring, sector); 0 where no point is."""
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        kind, tr = self._transforms(ids, poses6, affines)
+        out = np.empty((SC_RINGS, SC_SECTORS), np.float64)
+        _chk(lib().flb_keyframes_scan_context(self.h, _p(ids) if len(ids) else None, len(ids), kind, _p(tr) if len(ids) else None,
+                                              float(lidar_height), _p(out)))
+        return out
+
+    def scan_contexts(self, ids, lidar_height=1.5):
+        """makeScancontext of every key frame ids[j] as stored (the key-frame saver): (k, 20, 60) float64."""
+        ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+        out = np.empty((len(ids), SC_RINGS, SC_SECTORS), np.float64)
+        _chk(lib().flb_keyframes_scan_contexts(self.h, _p(ids) if len(ids) else None, len(ids), float(lidar_height),
+                                               _p(out) if len(ids) else None))
+        return out
 
 
 def make_fov(cube_len=200.0, det_range=100.0):

@@ -1772,3 +1772,4 @@ extern "C" int flb_debug_trace_read(unsigned long long* out, long long* phases, 
 #include "frontend_host.cuh"
 #include "preprocess_host.cuh"
 #include "keyframe_host.cuh"
+#include "scan_context_host.cuh"

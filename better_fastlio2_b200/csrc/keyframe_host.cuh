@@ -5,6 +5,7 @@
 // k_kf_assemble launch.  Included at the end of fastlio_b200.cu after frontend_host.cuh (uses VgWork, flb_frontend).
 #pragma once
 #include "keyframe_kernels.cuh"
+#include "scan_context_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------ map-side scratch
 // Kept with the map and only ever grown, like kf_raw / kf_in / kf_out: the readers run every kd_step key frames or on a
@@ -18,14 +19,19 @@ struct KfWork {
   KfSeg *d_seg = nullptr, *h_seg = nullptr;    // segment table of k_kf_assemble (device, pinned staging)
   int seg_cap = 0;
   cudaEvent_t ev_seg = nullptr;                // the last copy out of h_seg
+  ScChunk *d_chunk = nullptr, *h_chunk = nullptr;   // chunk table of k_sc_bins (device, pinned staging)
+  int chunk_cap = 0;
+  unsigned *d_sc_keys = nullptr, *h_sc_keys = nullptr;   // Scan Context keys, SC_BINS per descriptor (device, pinned)
+  int sc_cap = 0;                              // descriptors
 };
 
 static void kfw_release(KfWork* w) {
   if (!w) return;
   vg_release(w->vg);
-  void* ptrs[] = {w->cin, w->cout, w->d_seg};
+  void* ptrs[] = {w->cin, w->cout, w->d_seg, w->d_chunk, w->d_sc_keys};
   for (void* p : ptrs) if (p) Q(cudaFree(p));
-  if (w->h_seg) Q(cudaFreeHost(w->h_seg));
+  void* pinned[] = {w->h_seg, w->h_chunk, w->h_sc_keys};
+  for (void* p : pinned) if (p) Q(cudaFreeHost(p));
   if (w->ev_seg) Q(cudaEventDestroy(w->ev_seg));
   delete w;
 }
@@ -41,17 +47,22 @@ static int kf_grow(void** p, size_t* cap, size_t need) {
   return 0;
 }
 
+// The map's KfWork, created on first use.
+static int kf_work(flb_map* m) {
+  if (m->kfw) return 0;
+  cudaEvent_t ev = nullptr;
+  CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  m->kfw = new (std::nothrow) KfWork();
+  if (!m->kfw) { Q(cudaEventDestroy(ev)); return set_err("out of host memory"); }
+  m->kfw->ev_seg = ev;
+  return 0;
+}
+
 // Scratch for an assembly of n points: kf_in (the assembled cloud) and, when asked for, its curvature; with a filter
 // also kf_out (the filtered cloud), its curvature and the voxel-grid workspace.  A failure leaves the map's contents
 // untouched.
 static int kf_scratch(flb_map* m, int n, bool curv, bool filter) {
-  if (!m->kfw) {
-    cudaEvent_t ev = nullptr;
-    CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    m->kfw = new (std::nothrow) KfWork();
-    if (!m->kfw) { Q(cudaEventDestroy(ev)); return set_err("out of host memory"); }
-    m->kfw->ev_seg = ev;
-  }
+  if (kf_work(m)) return 1;
   KfWork& w = *m->kfw;
   const size_t pts = sizeof(float4) * (size_t)n, cur = sizeof(float) * (size_t)n;
   if (kf_grow((void**)&m->kf_in, &m->kf_in_cap, pts)) return 1;
@@ -66,6 +77,7 @@ static long long kf_scratch_bytes(const flb_map* m) {
   size_t b = m->kf_raw_cap + m->kf_in_cap + m->kf_out_cap;
   if (const KfWork* w = m->kfw) {
     b += w->cin_cap + w->cout_cap + sizeof(KfSeg) * (size_t)w->seg_cap;
+    b += sizeof(ScChunk) * (size_t)w->chunk_cap + sizeof(unsigned) * SC_BINS * (size_t)w->sc_cap;
     if (w->vg.cap) b += (2 * sizeof(unsigned) + 4 * sizeof(int)) * (size_t)w->vg.cap + w->vg.tmp_bytes + 8 * sizeof(unsigned);
   }
   return (long long)b;
@@ -107,10 +119,8 @@ static KfSeg kf_seg(const float* t12, bool copy, long long src_off, int dst_off,
   return s;
 }
 
-// One launch: out[dst_off + j] = segment transform of src[src_off + j] for every (non-empty) segment, in table order.
-static int kf_assemble_enqueue(flb_map* m, const std::vector<KfSeg>& segs, const float4* src, const float* src_curv, int n, float4* out,
-                               float* out_curv) {
-  if (n == 0) return 0;
+// The segment table into w.d_seg (through the pinned staging), on the map stream.
+static int kf_upload_segs(flb_map* m, const std::vector<KfSeg>& segs) {
   KfWork& w = *m->kfw;
   const int ns = (int)segs.size();
   CU(cudaEventSynchronize(w.ev_seg));   // the previous table copy has left the pinned staging
@@ -126,7 +136,16 @@ static int kf_assemble_enqueue(flb_map* m, const std::vector<KfSeg>& segs, const
   memcpy(w.h_seg, segs.data(), sizeof(KfSeg) * (size_t)ns);
   CU(cudaMemcpyAsync(w.d_seg, w.h_seg, sizeof(KfSeg) * (size_t)ns, cudaMemcpyHostToDevice, m->stream));
   CU(cudaEventRecord(w.ev_seg, m->stream));
-  k_kf_assemble<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.d_seg, ns, src, src_curv, n, out, out_curv);
+  return 0;
+}
+
+// One launch: out[dst_off + j] = segment transform of src[src_off + j] for every (non-empty) segment, in table order.
+static int kf_assemble_enqueue(flb_map* m, const std::vector<KfSeg>& segs, const float4* src, const float* src_curv, int n, float4* out,
+                               float* out_curv) {
+  if (n == 0) return 0;
+  if (kf_upload_segs(m, segs)) return 1;
+  k_kf_assemble<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->kfw->d_seg, (int)segs.size(), src, src_curv, n, out,
+                                                                          out_curv);
   m->launches++;
   CU(cudaGetLastError());
   return 0;
@@ -323,14 +342,19 @@ extern "C" int flb_keyframes_size(const flb_keyframes* k, int id) {
   return k->cnt[id];
 }
 
-// the selection's size, with every id checked (before any device work)
-static int kf_selection(const flb_keyframes* k, const int* ids, int n_ids, const char* who, int* total) {
-  long long t = 0;
-  for (int j = 0; j < n_ids; ++j) {
+// every id of a selection checked (before any device work)
+static int kf_check_ids(const flb_keyframes* k, const int* ids, int n_ids, const char* who) {
+  for (int j = 0; j < n_ids; ++j)
     if (ids[j] < 0 || ids[j] >= (int)k->cnt.size())
       return set_err("%s: key frame id %d (entry %d) out of range [0, %d)", who, ids[j], j, (int)k->cnt.size());
-    t += k->cnt[ids[j]];
-  }
+  return 0;
+}
+
+// the selection's size, with every id checked (before any device work)
+static int kf_selection(const flb_keyframes* k, const int* ids, int n_ids, const char* who, int* total) {
+  if (kf_check_ids(k, ids, n_ids, who)) return 1;
+  long long t = 0;
+  for (int j = 0; j < n_ids; ++j) t += k->cnt[ids[j]];
   if (t > INT_MAX) return set_err("%s: selection of %lld points is too large", who, t);
   *total = (int)t;
   return 0;
@@ -368,6 +392,26 @@ static bool is_identity(const float* t) {
   return true;
 }
 
+// The segment table of a selection: ids[j] with transforms[j] (FLB_KF_POSE6 / FLB_KF_AFFINE, the identity affine
+// copies), back to back from output point 0, empty key frames dropped.
+static void kf_selection_segs(const flb_keyframes* k, const int* ids, int n_ids, int transform_kind, const float* transforms,
+                              std::vector<KfSeg>& segs) {
+  segs.clear();
+  segs.reserve(n_ids);
+  int dst = 0;
+  for (int j = 0; j < n_ids; ++j) {
+    const int c = k->cnt[ids[j]];
+    if (c == 0) continue;
+    if (transform_kind == FLB_KF_POSE6) {
+      segs.push_back(kf_seg(affine_from_rpy(transforms + 6 * j).t, false, k->off[ids[j]], dst, c));
+    } else {
+      const float* t = transforms + 12 * j;
+      segs.push_back(kf_seg(t, is_identity(t), k->off[ids[j]], dst, c));
+    }
+    dst += c;
+  }
+}
+
 extern "C" int flb_keyframes_assemble(flb_keyframes* k, const int* ids, int n_ids, int transform_kind, const float* transforms, float leaf,
                                       float* out_xyzi, float* out_curvature, int cap, int* n_out) {
   if (!k) return set_err("null key-frame store");
@@ -384,19 +428,7 @@ extern "C" int flb_keyframes_assemble(flb_keyframes* k, const int* ids, int n_id
   if (kf_scratch(m, n, true, leaf > 0.f)) return 1;
   KfWork& w = *m->kfw;
   std::vector<KfSeg> segs;
-  segs.reserve(n_ids);
-  int dst = 0;
-  for (int j = 0; j < n_ids; ++j) {
-    const int c = k->cnt[ids[j]];
-    if (c == 0) continue;
-    if (transform_kind == FLB_KF_POSE6) {
-      segs.push_back(kf_seg(affine_from_rpy(transforms + 6 * j).t, false, k->off[ids[j]], dst, c));
-    } else {
-      const float* t = transforms + 12 * j;
-      segs.push_back(kf_seg(t, is_identity(t), k->off[ids[j]], dst, c));
-    }
-    dst += c;
-  }
+  kf_selection_segs(k, ids, n_ids, transform_kind, transforms, segs);
   if (kf_assemble_enqueue(m, segs, k->xyzi, k->curv, n, m->kf_in, w.cin)) return 1;
   if (leaf == 0.f) {   // the dense concatenation (GlobalMap.pcd, the loop sub-maps)
     if (n_out) *n_out = n;

@@ -17,28 +17,37 @@ struct KfSeg {
   int dst_off, count, copy, pad;
 };
 
-// Thread i writes output point i: its segment is the last one whose dst_off <= i (the host drops empty segments, so
-// dst_off is strictly increasing).  Neighbouring threads share a segment, so the search reads the same cached words.
+// Output point i's segment: the last one whose dst_off <= i (the host drops empty segments, so dst_off is strictly
+// increasing).  Neighbouring threads share a segment, so the search reads the same cached words.
+__device__ __forceinline__ const KfSeg* kf_seg_of(const KfSeg* __restrict__ segs, int n_seg, int i) {
+  int lo = 0, hi = n_seg - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (__ldg(&segs[mid].dst_off) <= i) lo = mid; else hi = mid - 1;
+  }
+  return segs + lo;
+}
+
+// Output point i of segment s: the stored record src[j] (copy) or its affine, x, y, z and intensity.  Every reader of a
+// selection (the assembly, the Scan Context bins) goes through this, so they all see the same points.
+__device__ __forceinline__ float4 kf_point(const KfSeg* s, const float4* __restrict__ src, int i, long long* j_out) {
+  const long long j = s->src_off + (i - s->dst_off);
+  *j_out = j;
+  const float4 p = src[j];
+  if (s->copy) return p;
+  const float* a = s->t;
+  return make_float4(a[0] * p.x + a[1] * p.y + a[2] * p.z + a[3], a[4] * p.x + a[5] * p.y + a[6] * p.z + a[7],
+                     a[8] * p.x + a[9] * p.y + a[10] * p.z + a[11], p.w);
+}
+
+// Thread i writes output point i.
 __global__ void k_kf_assemble(const KfSeg* __restrict__ segs, int n_seg, const float4* __restrict__ src, const float* __restrict__ src_curv,
                               int n, float4* __restrict__ out, float* __restrict__ out_curv) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    int lo = 0, hi = n_seg - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (__ldg(&segs[mid].dst_off) <= i) lo = mid; else hi = mid - 1;
-    }
-    const KfSeg* s = segs + lo;
-    const long long j = s->src_off + (i - s->dst_off);
-    const float4 p = src[j];
-    if (s->copy) {
-      out[i] = p;
-      if (out_curv) out_curv[i] = src_curv ? src_curv[j] : 0.f;
-    } else {
-      const float* a = s->t;
-      out[i] = make_float4(a[0] * p.x + a[1] * p.y + a[2] * p.z + a[3], a[4] * p.x + a[5] * p.y + a[6] * p.z + a[7],
-                           a[8] * p.x + a[9] * p.y + a[10] * p.z + a[11], p.w);
-      if (out_curv) out_curv[i] = 0.f;
-    }
+    const KfSeg* s = kf_seg_of(segs, n_seg, i);
+    long long j;
+    out[i] = kf_point(s, src, i, &j);
+    if (out_curv) out_curv[i] = (s->copy && src_curv) ? src_curv[j] : 0.f;
   }
 }
 

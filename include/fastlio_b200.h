@@ -389,6 +389,29 @@ int flb_keyframes_assemble(flb_keyframes* kf, const int* ids, int n_ids, int tra
  * all of it (waits for the map's stream); the next reader allocates again. */
 int flb_map_release_keyframe_scratch(flb_map* m);
 
+/* ------------------------------------------------------------------------------------------------ Scan Context
+ * SCManager::makeScancontext (include/sc-relo/Scancontext.cpp:195-251) of key-frame clouds in the store, computed where
+ * they are: each point is transformed exactly as flb_keyframes_assemble writes it, binned into one of 20 rings x 60
+ * sectors out to 80 m and max-reduced; only the descriptors come back.  Semantics are the reference's, types included:
+ * pt.z = (float)(z + lidar_height) in double; range = sqrtf(x*x + y*y) without FMA; the angle of xy2theta with a float
+ * quotient, double atan and degrees, rounded to float (x = -0, y > 0 gives -90 degrees, x = ±0, y = 0 NaN); a point is
+ * skipped when range > 80 (a NaN range is kept); ring / sector = clamp(ceil(...), 1, 20 / 60) in double, a NaN landing
+ * in index 1; a bin keeps the largest pt.z above -1000, a bin no point beat is 0.  Each descriptor is 20 x 60 doubles,
+ * row-major (ring, sector), every value exactly a float or 0.  The device's double atan is within 2 ulp of glibc's: a
+ * point whose angle lies within one float ulp of a 6-degree boundary can land in the neighbouring sector (DESIGN.md §5).
+ * Every argument is checked before any device work; one synchronisation per call; the store is not modified.  The chunk
+ * table and the descriptor keys are map-side key-frame scratch (flb_keyframes_info, flb_map_release_keyframe_scratch). */
+#define FLB_SC_RINGS 20     /* PC_NUM_RING, Scancontext.h:86 (const in the reference) */
+#define FLB_SC_SECTORS 60   /* PC_NUM_SECTOR, :87; PC_MAX_RADIUS 80 m, :88 */
+/* makeScancontext(loop sub-map of the selection) (performLoopClosure, laserMapping.cpp:932-933): ids in order, transforms
+ * as flb_keyframes_assemble (FLB_KF_POSE6 / FLB_KF_AFFINE, the identity copies), empty key frames dropped; out_desc = 20 x
+ * 60 doubles row-major.  n_ids == 0 (or only empty key frames): all zeros. */
+int flb_keyframes_scan_context(flb_keyframes* kf, const int* ids, int n_ids, int transform_kind, const float* transforms,
+                               double lidar_height, double* out_desc);
+/* makeScancontext(*surfCloudKeyFrames[ids[j]]) for every j, the stored records as they are (the saver, :2504-2505):
+ * out_descs = n_ids x 20 x 60 doubles; an empty key frame gives all zeros. */
+int flb_keyframes_scan_contexts(flb_keyframes* kf, const int* ids, int n_ids, double lidar_height, double* out_descs);
+
 /* Stream access for callers that overlap work (returns a cudaStream_t as void*). */
 void* flb_session_stream(flb_session* s);
 int flb_session_sync(flb_session* s);

@@ -12,6 +12,10 @@
 //   keyframes.assemble(ids, finalTrans, 0.f, *nearKeyframes);
 //   // the per-key-frame saver at shutdown (:2501-2505):
 //   keyframes.at(i, *save_cloud);
+//   // the Scan Context gate of performLoopClosure (:932-940), before any cloud is assembled: same ids and affines
+//   keyframes.scan_context(ids, finalTrans, scLoop.LIDAR_HEIGHT, cureKeyframeSC);
+//   // every key frame's descriptor for the saver (:2504-2505), then scLoop.saveScancontextAndKeys(descs[i])
+//   keyframes.scan_contexts(all_ids, scLoop.LIDAR_HEIGHT, descs);
 //
 // Poses6D is anything with points[k].{x, y, z, roll, pitch, yaw} (pcl::PointCloud<PointTypePose>); an affine is
 // anything with operator()(row, col) (Eigen::Affine3f).  Clouds come back with x, y, z, intensity and curvature set
@@ -102,11 +106,30 @@ class KeyFrameStore {
   template <class Affine, class Alloc, class Cloud>
   bool assemble(const std::vector<int>& ids, const std::vector<Affine, Alloc>& T, float leaf, Cloud& out) {
     if (T.size() != ids.size()) return ok(1, "assemble: one affine per key frame");
-    std::vector<float> t(ids.size() * 12);
-    for (size_t j = 0; j < ids.size(); ++j)
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 4; ++c) t[j * 12 + r * 4 + c] = T[j](r, c);
-    return run_assemble(ids, FLB_KF_AFFINE, t, leaf, out);
+    return run_assemble(ids, FLB_KF_AFFINE, affines12(T), leaf, out);
+  }
+
+  // scLoop.makeScancontext(*nearKeyframes) for the loop sub-map that assemble(ids, T, 0.f, ..) would return
+  // (performLoopClosure :932-933), computed on the device without assembling or downloading the cloud.  Mat is anything
+  // with resize(rows, cols) and operator()(row, col), i.e. Eigen::MatrixXd: 20 rings x 60 sectors.
+  template <class Affine, class Alloc, class Mat>
+  bool scan_context(const std::vector<int>& ids, const std::vector<Affine, Alloc>& T, double lidar_height, Mat& desc) {
+    if (T.size() != ids.size()) return ok(1, "scan_context: one affine per key frame");
+    return run_scan_context(ids, FLB_KF_AFFINE, affines12(T), lidar_height, desc);
+  }
+  // the same with the key frames' poses (poses.points[ids[j]])
+  template <class Poses6D, class Mat>
+  bool scan_context(const std::vector<int>& ids, const Poses6D& poses, double lidar_height, Mat& desc) {
+    return run_scan_context(ids, FLB_KF_POSE6, poses6(ids, poses), lidar_height, desc);
+  }
+  // makeScancontext(*surfCloudKeyFrames[ids[j]]) for every j (the key-frame saver, :2501-2505): descs[j], 20 x 60 each
+  template <class Mat, class Alloc>
+  bool scan_contexts(const std::vector<int>& ids, double lidar_height, std::vector<Mat, Alloc>& descs) {
+    sc_.resize(ids.size() * kScBins + 1);
+    if (!ok(flb_keyframes_scan_contexts(kf_, ids.data(), (int)ids.size(), lidar_height, sc_.data()), "scan_contexts")) return false;
+    descs.resize(ids.size());
+    for (size_t j = 0; j < ids.size(); ++j) to_mat(&sc_[j * kScBins], descs[j]);
+    return true;
   }
 
   // pcl::copyPointCloud(*surfCloudKeyFrames[k], out)
@@ -134,6 +157,28 @@ class KeyFrameStore {
       o[0] = q.x; o[1] = q.y; o[2] = q.z; o[3] = q.roll; o[4] = q.pitch; o[5] = q.yaw;
     }
     return p;
+  }
+  template <class Affine, class Alloc>
+  static std::vector<float> affines12(const std::vector<Affine, Alloc>& T) {
+    std::vector<float> t(T.size() * 12 + 12, 0.f);
+    for (size_t j = 0; j < T.size(); ++j)
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 4; ++c) t[j * 12 + r * 4 + c] = T[j](r, c);
+    return t;
+  }
+  template <class Mat>
+  bool run_scan_context(const std::vector<int>& ids, int kind, const std::vector<float>& t, double lidar_height, Mat& desc) {
+    sc_.resize(kScBins);
+    if (!ok(flb_keyframes_scan_context(kf_, ids.data(), (int)ids.size(), kind, t.data(), lidar_height, sc_.data()), "scan_context"))
+      return false;
+    to_mat(sc_.data(), desc);
+    return true;
+  }
+  template <class Mat>
+  static void to_mat(const double* d, Mat& m) {   // row-major (ring, sector)
+    m.resize(FLB_SC_RINGS, FLB_SC_SECTORS);
+    for (int r = 0; r < FLB_SC_RINGS; ++r)
+      for (int c = 0; c < FLB_SC_SECTORS; ++c) m(r, c) = d[r * FLB_SC_SECTORS + c];
   }
   int selection_size(const std::vector<int>& ids) const {
     long long t = 0;
@@ -170,7 +215,9 @@ class KeyFrameStore {
 
   flb_keyframes* kf_ = nullptr;
   flb_map* map_ = nullptr;
+  static const int kScBins = FLB_SC_RINGS * FLB_SC_SECTORS;
   std::vector<float> xyzi_, curv_;
+  std::vector<double> sc_;
 };
 
 }  // namespace flb
