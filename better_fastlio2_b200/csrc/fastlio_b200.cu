@@ -82,6 +82,14 @@ static inline int grid_for(int n, int threads, int max_blocks) {
   if (g < 1) g = 1;
   return g > max_blocks ? max_blocks : g;
 }
+// CTAs of `kern` that are resident on the whole device at once (the grid of a kernel that loops over its work)
+template <typename... P>
+static cudaError_t resident_ctas(void (*kern)(P...), int threads, size_t smem, int sm_count, int& out) {
+  int per_sm = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
+  out = std::max(per_sm, 1) * sm_count;
+  return e;
+}
 
 // ------------------------------------------------------------------------------------------------ map
 struct flb_map {
@@ -89,6 +97,7 @@ struct flb_map {
   flb_map_config cfg{};
   cudaStream_t stream = nullptr;
   int sm_count = 148;
+  int exact_ctas[2] = {0, 0};    // resident CTAs of k_knn<5>, <20> (the grid of the exact completion)
   uint32_t hash_cap = 0, chash_cap = 0;
   size_t device_bytes = 0;
   bool has_root = false;
@@ -218,6 +227,8 @@ extern "C" int flb_map_create(const flb_map_config* cfg, flb_map** out) {
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, cfg->device));
   m->sm_count = prop.multiProcessorCount;
+  CU(resident_ctas(k_knn<5>, KNN_THREADS, 0, m->sm_count, m->exact_ctas[0]));
+  CU(resident_ctas(k_knn<20>, KNN_THREADS, 0, m->sm_count, m->exact_ctas[1]));
   if (const char* g = getenv("FLB_KNN_GROUP")) m->knn_group = (atoi(g) == 8) ? 8 : 32;
   CU(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
   MapDev& d = m->d;
@@ -526,10 +537,13 @@ static int launch_knn(flb_map* m, KnnArgs a) {
     a.work_ticket = m->d_misc + 13;
     CU(cudaMemsetAsync(a.work_count, 0, 2 * sizeof(int), m->stream));
   }
+  // one thread per query (a.n is the session capacity on the device-driven path; CTAs past the scan's size exit at once).
+  // A cfg2 scan (~930 CTAs) is a little more than the 924 CTAs an H100 holds at 7 per SM.  Two ways to make it one wave
+  // were measured slower (DESIGN.md §3): a resident grid looping over warp-sized chunks claimed by ticket (the loop cost
+  // ~250 B of register spills per thread) and a 64-register cap for 8 CTAs per SM (~100 B of spills).
   launch_k(k_knn_stencil<K>, (a.n + 127) / 128, 128, 0, m->stream, a);
-  // the fallback grid is sized for the typical <2 % unresolved share; it loops over the list
-  // all CTAs resident; they loop over the list.  Lanes per query: 8 (four queries per warp) or a whole warp
-  launch_k(k_knn<K>, m->sm_count * KNN_MIN_CTAS, KNN_THREADS, 0, m->stream, a);
+  // the exact completion: all CTAs resident (from the occupancy API), looping over the work list
+  launch_k(k_knn<K>, m->exact_ctas[K == 5 ? 0 : 1], KNN_THREADS, 0, m->stream, a);
   m->launches += 2;
   return 0;
 }
@@ -913,9 +927,13 @@ extern "C" int flb_session_create(flb_map* m, const flb_session_config* cfg, flb
   s->cfg = *cfg;
   s->cap = cfg->max_scan_points;
   const size_t N = (size_t)s->cap;
-  s->res_grid = m->sm_count;
   cudaError_t e = cudaFuncSetAttribute(k_residual<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, meas_smem_bytes<true>());   // > 48 KB
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_residual<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, meas_smem_bytes<false>());
+  // one partial per resident CTA (one per SM); the partial buffer and the final reductions follow
+  if (e == cudaSuccess) {
+    if (cfg->extrinsic_est_en) e = resident_ctas(k_residual<true>, meas_threads<true>(), meas_smem_bytes<true>(), m->sm_count, s->res_grid);
+    else e = resident_ctas(k_residual<false>, meas_threads<false>(), meas_smem_bytes<false>(), m->sm_count, s->res_grid);
+  }
   auto A = [&](void** p, size_t b) { if (e == cudaSuccess) e = cudaMalloc(p, b); };
   A((void**)&s->body, sizeof(float4) * N);
   A((void**)&s->body_alt, sizeof(float4) * N);
@@ -1176,8 +1194,8 @@ static int enqueue_pass(flb_session* s, const double* state26, int search) {
   const MeasArgs ma = meas_args(s, pose, search);
   {
     ProfScope ps(m, FLB_K_RESIDUAL);
-    if (s->cfg.extrinsic_est_en) k_residual<true><<<s->res_grid, MEAS_THREADS, meas_smem_bytes<true>(), st>>>(ma);
-    else k_residual<false><<<s->res_grid, MEAS_THREADS, meas_smem_bytes<false>(), st>>>(ma);
+    if (s->cfg.extrinsic_est_en) k_residual<true><<<s->res_grid, meas_threads<true>(), meas_smem_bytes<true>(), st>>>(ma);
+    else k_residual<false><<<s->res_grid, meas_threads<false>(), meas_smem_bytes<false>(), st>>>(ma);
     m->launches++;
   }
   {
@@ -1355,8 +1373,8 @@ static int enqueue_scan_device(flb_session* s, bool with_insert) {
       ProfScope ps(m, FLB_K_RESIDUAL);
       MeasArgs ma = meas_args(s, PoseDev{}, 0);
       ma.ctl = s->ctl;
-      if (s->cfg.extrinsic_est_en) launch_k(k_residual<true>, s->res_grid, MEAS_THREADS, meas_smem_bytes<true>(), st, ma);
-      else launch_k(k_residual<false>, s->res_grid, MEAS_THREADS, meas_smem_bytes<false>(), st, ma);
+      if (s->cfg.extrinsic_est_en) launch_k(k_residual<true>, s->res_grid, meas_threads<true>(), meas_smem_bytes<true>(), st, ma);
+      else launch_k(k_residual<false>, s->res_grid, meas_threads<false>(), meas_smem_bytes<false>(), st, ma);
       m->launches++;
     }
     if (overlap) CU(cudaStreamWaitEvent(st, s->ev_join[p], 0));

@@ -671,7 +671,7 @@ __device__ __forceinline__ unsigned long long stencil_mask(unsigned ax, unsigned
 }
 
 // Per-thread shared-memory columns of the stencil kernel: 220 B per query, so that 7 CTAs of 128 threads (the register
-// limit) fit one SM: 118 272 queries per wave on an H100's 132 SMs, about one 120k-point scan.
+// limit) fit one SM: 118 272 queries per wave on an H100's 132 SMs, slightly less than a cfg2 scan (118-119k points).
 struct StencilSmem {
   int blk[8][STENCIL_THREADS];                     // block index of the 8 probed blocks (-1: absent)
   unsigned long long c5[8][STENCIL_THREADS];       // occupied voxels of each block inside the 5x5x5 stencil

@@ -163,13 +163,17 @@ __device__ __forceinline__ bool esti_plane_dev(const float (&P)[5][3], float thr
 }
 
 // ---------------------------------------------------------------------------------------------- K1': residual + H^T H
-// One CTA per SM (one block partial per SM for the update kernel to reduce; at 72 registers the register file holds one
-// such CTA).  896 threads = 118 272 over an H100's 132 SMs: all but the last ~1 % of a 120k-point scan in ONE round of the
-// point loop (512 threads need two full rounds); the price is a 72-register cap (a few spilled values in the QR).
+// One CTA per SM (one block partial per SM for the update kernel to reduce; the register file holds one such CTA).
+// Without extrinsic estimation: 1024 threads = 135 168 over an H100's 132 SMs, so a scan of up to 131 072 points (the
+// default session capacity) runs in ONE round of the point loop and no CTA works through a second round while the rest of
+// the grid waits at the end; the price is a 64-register cap (a few spilled values in the QR).  With extrinsic estimation
+// (13-wide rows) 896 threads at a 72-register cap: at 1024 threads the extra spills made cfg3 (240k-point scans, several
+// rounds either way) 3.5 % slower on an H100.
 #ifndef FLB_MEAS_THREADS
-#define FLB_MEAS_THREADS 896
+#define FLB_MEAS_THREADS 1024
 #endif
-constexpr int MEAS_THREADS = FLB_MEAS_THREADS;
+template <bool EXTR>
+__host__ __device__ constexpr int meas_threads() { return EXTR ? 896 : FLB_MEAS_THREADS; }
 constexpr int NACC = 93;  // 91 upper-triangular entries of [h_x | h]^T [h_x | h] (13x13) + total_residual + M
 
 struct MeasArgs {
@@ -261,10 +265,10 @@ __device__ __forceinline__ bool select_point(const MeasArgs& a, int i, int searc
 }
 
 template <bool EXTR>
-constexpr int meas_smem_bytes() { return (MEAS_THREADS / 32) * 32 * (EXTR ? 13 : 7) * (int)sizeof(double); }
+constexpr int meas_smem_bytes() { return (meas_threads<EXTR>() / 32) * 32 * (EXTR ? 13 : 7) * (int)sizeof(double); }
 
 template <bool EXTR>
-__global__ void __launch_bounds__(MEAS_THREADS) k_residual(MeasArgs a) {
+__global__ void __launch_bounds__(meas_threads<EXTR>()) k_residual(MeasArgs a) {
   pdl_sync();
   constexpr int W = EXTR ? 13 : 7;               // augmented row width [cols..., h]
   constexpr int NE = W * (W + 1) / 2;            // 91 or 28
@@ -362,7 +366,7 @@ __global__ void __launch_bounds__(MEAS_THREADS) k_residual(MeasArgs a) {
   __syncthreads();
   for (int e = threadIdx.x; e < NACC; e += blockDim.x) {
     double s = 0.0;
-    for (int w = 0; w < MEAS_THREADS / 32; ++w) s += wacc[w][e];
+    for (int w = 0; w < meas_threads<EXTR>() / 32; ++w) s += wacc[w][e];
     a.partial[(size_t)blockIdx.x * NACC + e] = s;
   }
   FLB_TRACE_END(4 * 8 + (a.ctl ? a.ctl->it + 1 : 0));
