@@ -189,9 +189,10 @@ struct State {
   }
 };
 
-// Dense inverse with partial pivoting (role of Eigen's PartialPivLU-based .inverse(), esekfom.hpp:1788,1808).
-template <int N>
-inline bool inverse(const Mat<N, N>& A, Mat<N, N>& Ai) {
+// LU factorisation with partial pivoting (Eigen's PartialPivLU, esekfom.hpp:1788,1808), then X = A^-1 B for the C
+// columns of B.  B = I gives the dense inverse.
+template <int N, int C>
+inline bool lu_solve(const Mat<N, N>& A, const Mat<N, C>& B, Mat<N, C>& X) {
   Mat<N, N> lu = A;
   int piv[N];
   for (int i = 0; i < N; ++i) piv[i] = i;
@@ -207,22 +208,24 @@ inline bool inverse(const Mat<N, N>& A, Mat<N, N>& Ai) {
       if (f != 0.0) for (int j = c + 1; j < N; ++j) lu(r, j) -= f * lu(c, j);
     }
   }
-  // solve LU X = P I column by column
-  for (int col = 0; col < N; ++col) {
+  // solve LU X = P B column by column
+  for (int col = 0; col < C; ++col) {
     double y[N];
     for (int i = 0; i < N; ++i) {
-      double s = (piv[i] == col) ? 1.0 : 0.0;
+      double s = B(piv[i], col);
       for (int k = 0; k < i; ++k) s -= lu(i, k) * y[k];
       y[i] = s;
     }
     for (int i = N - 1; i >= 0; --i) {
       double s = y[i];
-      for (int k = i + 1; k < N; ++k) s -= lu(i, k) * Ai(k, col);
-      Ai(i, col) = s / lu(i, i);
+      for (int k = i + 1; k < N; ++k) s -= lu(i, k) * X(k, col);
+      X(i, col) = s / lu(i, i);
     }
   }
   return true;
 }
+template <int N>
+inline bool inverse(const Mat<N, N>& A, Mat<N, N>& Ai) { return lu_solve(A, Mat<N, N>::identity(), Ai); }
 
 // Block helpers: rows [idx, idx+D) <- J * Src rows ; cols [idx, idx+D) <- cols * J^T.
 template <int D>
@@ -259,21 +262,25 @@ class IteratedUpdate {
 
   // One pass with a valid measurement (M >= 1): HTH 12x12 row-major, HTh 12.  Requires M >= DOF for the
   // information-form branch (esekfom.hpp:1788-1815); the rare M < 23 branch needs the rows (see step_rows).
+  // [K_x[:, 0:12] | K_h] = P_temp^-1 [H^T H | H^T h] (rows 12.. zero) is SOLVED from P_temp's LU factors instead of
+  // forming P_temp^-1 and multiplying as the reference does: with extrinsic estimation P_temp is ill-conditioned
+  // (position and extrinsic translation enter the rows almost alike) and the explicit inverse times the large H^T H
+  // loses digits (6.6e-10 in the state against a float64 solve on a dense prior, tests/test_esikf_dense_cpu.py).
   void step(const double* HTH, const double* HTh) {
     double dx[DOF];
     prepare(dx);
     Cov PR;
     for (int i = 0; i < DOF * DOF; ++i) PR.a[i] = P_.a[i] / R_;
-    Cov P_temp, P_inv;
+    Cov P_temp;
     inverse(PR, P_temp);
     for (int a = 0; a < 12; ++a) for (int b = 0; b < 12; ++b) P_temp(a, b) += HTH[a * 12 + b];
-    inverse(P_temp, P_inv);
+    Mat<DOF, 13> rhs = Mat<DOF, 13>::zero(), sol;
+    for (int a = 0; a < 12; ++a) { for (int b = 0; b < 12; ++b) rhs(a, b) = HTH[a * 12 + b]; rhs(a, 12) = HTh[a]; }
+    lu_solve(P_temp, rhs, sol);
     K_x_ = Cov::zero();
     for (int i = 0; i < DOF; ++i) {
-      double s = 0;
-      for (int k = 0; k < 12; ++k) s += P_inv(i, k) * HTh[k];
-      K_h_[i] = s;
-      for (int b = 0; b < 12; ++b) { double q = 0; for (int k = 0; k < 12; ++k) q += P_inv(i, k) * HTH[k * 12 + b]; K_x_(i, b) = q; }
+      K_h_[i] = sol(i, 12);
+      for (int b = 0; b < 12; ++b) K_x_(i, b) = sol(i, b);
     }
     finish(dx);
   }

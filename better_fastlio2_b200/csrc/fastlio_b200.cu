@@ -919,6 +919,8 @@ extern "C" void flb_session_default_config(flb_session_config* c) {
 extern "C" int flb_session_create(flb_map* m, const flb_session_config* cfg, flb_session** out) {
   if (!m || !cfg || !out) return set_err("flb_session_create: null argument");
   if (cfg->max_scan_points <= 0) return set_err("max_scan_points must be > 0");
+  // the scan sequence holds one pass per iteration plus the first (esekfom.hpp:1636 runs i = -1 .. max_iter-1), at most 8
+  if (cfg->max_iterations < 0 || cfg->max_iterations > 7) return set_err("max_iterations must be in 0..7, got %d", cfg->max_iterations);
   CU(cudaSetDevice(m->cfg.device));
   flb_session* s = new (std::nothrow) flb_session();
   if (!s) return set_err("out of host memory");
@@ -960,7 +962,6 @@ extern "C" int flb_session_create(flb_map* m, const flb_session_config* cfg, flb
     e = cudaEventCreateWithFlags(&s->ev_fork[i], cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->ev_join[i], cudaEventDisableTiming);
   }
-  if (e == cudaSuccess && cfg->max_iterations + 1 > 8) { flb_session_destroy(s); return set_err("max_iterations must be <= 7"); }
   if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_out, sizeof(double) * NACC);
   if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_cnt2, sizeof(int) * 8);
   if (e == cudaSuccess) e = cudaEventCreate(&s->ev0);
