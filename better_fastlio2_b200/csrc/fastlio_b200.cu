@@ -4,12 +4,14 @@
 #include "../../include/fastlio_b200.h"
 #include "map_kernels.cuh"
 #include "knn_kernels.cuh"
+#include "frontend_kernels.cuh"
 #include "meas_kernels.cuh"
 #include "esikf_device.cuh"
 #include "knn_tile.cuh"
 #include "esikf_host.hpp"
 
 #include <cub/device/device_scan.cuh>
+#include <algorithm>
 #include <chrono>
 #include <climits>
 #include <cstdarg>
@@ -44,6 +46,40 @@ static void quiet(cudaError_t e, const char* what) {
   }
 }
 #define Q(call) quiet((call), #call)
+
+// ------------------------------------------------------------------------------------------------ grow-only buffers
+// Scratch that is only ever grown and whose contents need not survive a growth.  grow() frees the old allocation, then
+// allocates max(need, floor) bytes; a failure leaves the buffer empty.  Every caller keeps its own floor (or headroom):
+// how often a buffer is reallocated decides how often the captured scan graphs are re-captured (flb_map::gen).  The
+// owner frees it by destroying it, with its device current.
+template <typename T, bool Pinned>
+struct GrowBuf {
+  T* p = nullptr;
+  size_t cap = 0;   // bytes
+  GrowBuf() = default;
+  GrowBuf(const GrowBuf&) = delete;
+  GrowBuf& operator=(const GrowBuf&) = delete;
+  ~GrowBuf() { release(); }
+  void release() {
+    if (p) Q(Pinned ? cudaFreeHost(p) : cudaFree(p));
+    p = nullptr;
+    cap = 0;
+  }
+};
+template <typename T> using DevBuf = GrowBuf<T, false>;
+template <typename T> using PinnedBuf = GrowBuf<T, true>;   // page-locked host staging
+
+template <typename T, bool Pinned>
+static int grow(GrowBuf<T, Pinned>& b, size_t need, size_t floor) {
+  if (need <= b.cap) return 0;
+  b.release();
+  const size_t cap = std::max(need, floor);
+  void* p = nullptr;
+  CU(Pinned ? cudaMallocHost(&p, cap) : cudaMalloc(&p, cap));
+  b.p = static_cast<T*>(p);
+  b.cap = cap;
+  return 0;
+}
 
 extern "C" const char* flb_last_error(void) { return g_err; }
 extern "C" const char* flb_version(void) { return "fastlio_b200 0.1 (sm_90a)"; }
@@ -103,17 +139,12 @@ struct flb_map {
   bool has_root = false;
   int rehash_count = 0;
   // staging
-  float4* stage = nullptr;       // device float4 staging for host uploads
-  int stage_cap = 0;
-  unsigned char* raw = nullptr;  // device raw strided upload buffer
-  size_t raw_cap = 0;
-  uint64_t* skeys = nullptr;     // scratch hash of the downsampled insert
-  unsigned long long* sbest = nullptr;
-  uint32_t scratch_cap = 0;
-  float* dparams = nullptr;      // small device parameter buffer (boxes / points)
-  int dparams_cap = 0;
-  float4* outbuf = nullptr;      // collect output
-  int outbuf_cap = 0;
+  DevBuf<float4> stage;          // device float4 staging for host uploads
+  DevBuf<unsigned char> raw;     // device raw strided upload buffer
+  DevBuf<uint64_t> skeys;        // scratch hash of the downsampled insert (scratch_slots entries)
+  DevBuf<unsigned long long> sbest;
+  DevBuf<float> dparams;         // small device parameter buffer (boxes / points)
+  DevBuf<float4> outbuf;         // collect output
   int* h_counters = nullptr;     // pinned mirror of counters
   int* d_misc = nullptr;         // misc device ints (out counts, range)
   int launches = 0;              // kernel launch counter (cumulative)
@@ -125,18 +156,14 @@ struct flb_map {
   std::vector<ProfRec> prof_pool;
   size_t prof_used = 0;
   int* d_phase = nullptr;        // k-NN phase histogram (device, 4 ints)
-  int* worklist = nullptr;       // unresolved-query list of the stencil k-NN kernel
-  int work_cap = 0;
+  DevBuf<int> worklist;          // unresolved-query list of the stencil k-NN kernel
   bool scratch_clean = false;    // the downsample scratch hash was already cleared off the critical path (scan graph)
-  unsigned char* kf_raw = nullptr;   // flb_map_reconstruct_keyframes scratch (grow-only)
-  float4 *kf_in = nullptr, *kf_out = nullptr;
-  size_t kf_raw_cap = 0, kf_in_cap = 0, kf_out_cap = 0;   // bytes
+  DevBuf<unsigned char> kf_raw;  // flb_map_reconstruct_keyframes scratch
+  DevBuf<float4> kf_in, kf_out;
   struct KfWork* kfw = nullptr;      // the rest of the key-frame readers' scratch (keyframe_host.cuh, grow-only)
   int gen = 0;                   // bumped whenever a buffer or parameter baked into a captured scan graph changes (scratch hash,
                                  // work list, voxel size): sessions re-capture their graphs on a mismatch
   bool warned_range = false;
-  int knn_group = 32;            // lanes per query of the exact k-NN kernel: a whole warp; FLB_KNN_GROUP=8 selects four
-                                 // queries per warp (tuning only)
 };
 
 struct ProfScope {
@@ -229,7 +256,6 @@ extern "C" int flb_map_create(const flb_map_config* cfg, flb_map** out) {
   m->sm_count = prop.multiProcessorCount;
   CU(resident_ctas(k_knn<5>, KNN_THREADS, 0, m->sm_count, m->exact_ctas[0]));
   CU(resident_ctas(k_knn<20>, KNN_THREADS, 0, m->sm_count, m->exact_ctas[1]));
-  if (const char* g = getenv("FLB_KNN_GROUP")) m->knn_group = (atoi(g) == 8) ? 8 : 32;
   CU(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
   MapDev& d = m->d;
   d.ds = cfg->voxel_size;
@@ -282,7 +308,7 @@ static void map_release(flb_map* m) {
   if (m->stream) Q(cudaStreamSynchronize(m->stream));
   MapDev& d = m->d;
   void* ptrs[] = {d.clist, d.hent, d.bslot, d.slots, d.sint, d.oint, d.ovf, d.bkey, d.brel, d.free_blk, d.free_ovf, d.ckeys, d.cbits, d.counters,
-                  m->d_misc, m->stage, m->raw, m->skeys, m->sbest, m->dparams, m->outbuf, m->d_phase, m->worklist, m->kf_raw, m->kf_in, m->kf_out};
+                  m->d_misc, m->d_phase};
   for (void* p : ptrs) if (p) Q(cudaFree(p));
   if (m->h_counters) Q(cudaFreeHost(m->h_counters));
   kfw_release(m->kfw);
@@ -305,52 +331,63 @@ extern "C" int flb_map_set_downsample_param(flb_map* m, float v) {
 }
 extern "C" int flb_map_has_root(const flb_map* m) { return m && m->has_root ? 1 : 0; }
 
-// host strided points -> device float4 staging (x, y, z, intensity).  off_i: byte offset of the intensity inside a record,
-// < 0 = none (0).  16-byte records are taken as (x, y, z, intensity) verbatim.
-static int upload_points(flb_map* m, const void* pts, int n, int stride, int off_i = -1) {
-  if (n <= 0) return 0;
-  if (!pts) return set_err("null point buffer");
-  if (stride < 12) return set_err("stride_bytes must be >= 12");
-  if (off_i >= 0 && off_i + 4 > stride) return set_err("intensity offset %d outside the %d-byte record", off_i, stride);
-  if (n > m->stage_cap) {
-    if (m->stage) cudaFree(m->stage);
-    m->stage = nullptr;
-    m->stage_cap = 0;
-    int cap = std::max(n, 1 << 16);
-    CU(cudaMalloc((void**)&m->stage, sizeof(float4) * (size_t)cap));
-    m->stage_cap = cap;
-  }
-  if (stride == 16 && (off_i < 0 || off_i == 12)) {
-    CU(cudaMemcpyAsync(m->stage, pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
-    return 0;
-  }
-  const size_t bytes = (size_t)(n - 1) * stride + (size_t)std::max(12, off_i + 4);
-  if (bytes > m->raw_cap) {
-    if (m->raw) cudaFree(m->raw);
-    m->raw = nullptr;
-    m->raw_cap = 0;
-    size_t cap = std::max(bytes, (size_t)1 << 20);
-    CU(cudaMalloc((void**)&m->raw, cap));
-    m->raw_cap = cap;
-  }
-  CU(cudaMemcpyAsync(m->raw, pts, bytes, cudaMemcpyHostToDevice, m->stream));
-  k_pack_points<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->raw, stride, off_i, m->stage, n);
+// n > 0 records of `stride` bytes, already on the device at `raw` -> dst (x, y, z, intensity at byte off_i) and, when curv is
+// given, curv (curvature at off_c); a negative offset means the field is absent (0).  On `st`.
+static int pack_records(flb_map* m, cudaStream_t st, const unsigned char* raw, int n, int stride, int off_i, int off_c, float4* dst,
+                        float* curv) {
+  k_pack_xyzic<<<grid_for(n, 256, m->sm_count * 8), 256, 0, st>>>(raw, stride, off_i, off_c, dst, curv, n);
   m->launches++;
   CU(cudaGetLastError());
   return 0;
 }
 
-static int ensure_scratch(flb_map* m, int n) {
-  uint32_t need = next_pow2((uint64_t)std::max(n, 512) * 2);
-  if (need > m->scratch_cap) {
-    if (m->skeys) cudaFree(m->skeys);
-    if (m->sbest) cudaFree(m->sbest);
-    m->skeys = nullptr; m->sbest = nullptr; m->scratch_cap = 0;
-    CU(cudaMalloc((void**)&m->skeys, sizeof(uint64_t) * need));
-    CU(cudaMalloc((void**)&m->sbest, sizeof(unsigned long long) * need));
-    m->scratch_cap = need;
-    m->gen++;
+// n > 0 host records -> device, staged in `raw` (grown to at least raw_floor bytes) and packed as pack_records does, on `st`.
+// Records that are (x, y, z, intensity) already (16 bytes, intensity at 12, no curvature asked for) are copied straight to
+// dst: no staging, no launch.  Entry points that read a 16-byte record's 4th float as its intensity pass off_i = 12.
+static int upload_records(flb_map* m, cudaStream_t st, DevBuf<unsigned char>& raw, size_t raw_floor, const void* src, int n, int stride,
+                          int off_i, int off_c, float4* dst, float* curv) {
+  if (stride == 16 && off_i == 12 && !curv) {
+    CU(cudaMemcpyAsync(dst, src, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, st));
+    return 0;
   }
+  if (!curv) off_c = -1;
+  // the last record is read only up to the end of its last field used
+  const size_t bytes = (size_t)(n - 1) * stride + (size_t)std::max({12, off_i + 4, off_c + 4});
+  if (grow(raw, bytes, raw_floor)) return 1;
+  CU(cudaMemcpyAsync(raw.p, src, bytes, cudaMemcpyHostToDevice, st));
+  return pack_records(m, st, raw.p, n, stride, off_i, off_c, dst, curv);
+}
+
+// host strided points -> m->stage (x, y, z, intensity).  off_i: byte offset of the intensity inside a record, < 0 = none
+// (0).  16-byte records are taken as (x, y, z, intensity) verbatim.
+static int upload_points(flb_map* m, const void* pts, int n, int stride, int off_i = -1) {
+  if (n <= 0) return 0;
+  if (!pts) return set_err("null point buffer");
+  if (stride < 12) return set_err("stride_bytes must be >= 12");
+  if (off_i >= 0 && off_i + 4 > stride) return set_err("intensity offset %d outside the %d-byte record", off_i, stride);
+  if (stride == 16 && off_i < 0) off_i = 12;
+  if (grow(m->stage, sizeof(float4) * (size_t)n, sizeof(float4) << 16)) return 1;
+  return upload_records(m, m->stream, m->raw, (size_t)1 << 20, pts, n, stride, off_i, -1, m->stage.p, nullptr);
+}
+
+// entries of the downsampled insert's scratch hash for n points (load factor <= 1/2)
+static inline uint32_t scratch_slots(int n) { return next_pow2((uint64_t)std::max(n, 512) * 2); }
+
+// the scratch hash (skeys / sbest) for n points; a captured scan graph holds its address
+static int ensure_scratch(flb_map* m, int n) {
+  const size_t need = sizeof(uint64_t) * scratch_slots(n);
+  if (need <= m->skeys.cap && need <= m->sbest.cap) return 0;
+  if (grow(m->skeys, need, 0) || grow(m->sbest, need, 0)) return 1;
+  m->gen++;
+  return 0;
+}
+
+// the stencil k-NN kernel's work list for n queries; a captured scan graph holds its address
+static int ensure_worklist(flb_map* m, int n) {
+  const size_t need = sizeof(int) * (size_t)n;
+  if (need <= m->worklist.cap) return 0;
+  if (grow(m->worklist, need, sizeof(int) << 17)) return 1;
+  m->gen++;
   return 0;
 }
 
@@ -372,18 +409,18 @@ static int insert_device(flb_map* m, const float4* pts, const unsigned char* cls
     m->launches++;
   }
   if (mode == 1 || mode == 2) {
-    const uint32_t sc = next_pow2((uint64_t)std::max(n, 512) * 2);
+    const uint32_t sc = scratch_slots(n);
     if (!prefused) {
       if (ensure_scratch(m, n)) return 1;
       if (!m->scratch_clean) {
-        CU(cudaMemsetAsync(m->skeys, 0xFF, sizeof(uint64_t) * sc, st));
-        CU(cudaMemsetAsync(m->sbest, 0xFF, sizeof(unsigned long long) * sc, st));
+        CU(cudaMemsetAsync(m->skeys.p, 0xFF, sizeof(uint64_t) * sc, st));
+        CU(cudaMemsetAsync(m->sbest.p, 0xFF, sizeof(unsigned long long) * sc, st));
       }
-      launch_k(k_ds_scatter, g, 256, 0, st, m->d, pts, c, n, m->skeys, m->sbest, sc - 1, skip, n_dev);
+      launch_k(k_ds_scatter, g, 256, 0, st, m->d, pts, c, n, m->skeys.p, m->sbest.p, sc - 1, skip, n_dev);
       m->launches++;
     }
     m->scratch_clean = false;
-    launch_k(k_ds_apply, g, 256, 0, st, m->d, pts, c, n, (const uint64_t*)m->skeys, (const unsigned long long*)m->sbest, sc - 1, skip, n_dev);
+    launch_k(k_ds_apply, g, 256, 0, st, m->d, pts, c, n, (const uint64_t*)m->skeys.p, (const unsigned long long*)m->sbest.p, sc - 1, skip, n_dev);
     m->launches++;
   }
   if (mode == 0 || mode == 2) {
@@ -415,7 +452,7 @@ extern "C" int flb_map_build_pt(flb_map* m, const void* pts, int n, int stride, 
   if (map_reset_storage(m)) return 1;
   if (n == 0) return 0;  // Build with an empty cloud leaves Root_Node == nullptr (ikd_Tree.cpp:357)
   if (upload_points(m, pts, n, stride, off_intensity)) return 1;
-  if (insert_device(m, m->stage, nullptr, n, 0)) return 1;
+  if (insert_device(m, m->stage.p, nullptr, n, 0)) return 1;
   return fetch_counters(m);
 }
 extern "C" int flb_map_build(flb_map* m, const float* xyz, int n, int stride) { return flb_map_build_pt(m, xyz, n, stride, -1); }
@@ -431,7 +468,7 @@ extern "C" int flb_map_add_points_pt(flb_map* m, const void* pts, int n, int str
   CU(cudaSetDevice(m->cfg.device));
   if (upload_points(m, pts, n, stride, off_intensity)) return 1;
   if (zero_scratch_counters(m)) return 1;
-  if (insert_device(m, m->stage, nullptr, n, downsample_on ? 1 : 0)) return 1;
+  if (insert_device(m, m->stage.p, nullptr, n, downsample_on ? 1 : 0)) return 1;
   if (fetch_counters(m)) return 1;
   // reference return value: tmp_counter counts downsample add ops only (ikd_Tree.cpp:447,457,488)
   if (n_added) *n_added = downsample_on ? m->h_counters[CNT_SCRATCH0] : 0;
@@ -442,14 +479,8 @@ extern "C" int flb_map_add_points(flb_map* m, const float* xyz, int n, int strid
 }
 
 static int upload_params(flb_map* m, const float* host, int nfloats) {
-  if (nfloats > m->dparams_cap) {
-    if (m->dparams) cudaFree(m->dparams);
-    m->dparams = nullptr; m->dparams_cap = 0;
-    int cap = std::max(nfloats, 256);
-    CU(cudaMalloc((void**)&m->dparams, sizeof(float) * cap));
-    m->dparams_cap = cap;
-  }
-  CU(cudaMemcpyAsync(m->dparams, host, sizeof(float) * nfloats, cudaMemcpyHostToDevice, m->stream));
+  if (grow(m->dparams, sizeof(float) * (size_t)nfloats, sizeof(float) * 256)) return 1;
+  CU(cudaMemcpyAsync(m->dparams.p, host, sizeof(float) * nfloats, cudaMemcpyHostToDevice, m->stream));
   return 0;
 }
 
@@ -471,7 +502,7 @@ static int delete_common(flb_map* m, const float* params, int np, int floats_per
   const int g = grid_for(nblk * 32, 256, m->sm_count * 8);
   {
     ProfScope ps(m, FLB_K_DELETE);
-    k_delete<<<g, 256, 0, m->stream>>>(m->d, m->dparams, np, mode, nblk);
+    k_delete<<<g, 256, 0, m->stream>>>(m->d, m->dparams.p, np, mode, nblk);
     m->launches++;
   }
   CU(cudaGetLastError());
@@ -522,15 +553,8 @@ static int maybe_rehash(flb_map* m) {
 // k-NN = thread-per-query stencil kernel + exact warp-per-query kernel over the (small) unresolved work list.
 template <int K>
 static int launch_knn(flb_map* m, KnnArgs a) {
-  if (a.n > m->work_cap) {
-    if (m->worklist) cudaFree(m->worklist);
-    m->worklist = nullptr; m->work_cap = 0;
-    const int cap = std::max(a.n, 1 << 17);
-    CU(cudaMalloc((void**)&m->worklist, sizeof(int) * (size_t)cap));
-    m->work_cap = cap;
-    m->gen++;
-  }
-  a.worklist = m->worklist;
+  if (ensure_worklist(m, a.n)) return 1;
+  a.worklist = m->worklist.p;
   if (a.stride <= 0) a.stride = a.n;
   if (!a.work_count) {   // (device-driven scans use per-pass counters zeroed by k_esikf_begin: no memset node per pass)
     a.work_count = m->d_misc + 12;
@@ -548,16 +572,7 @@ static int launch_knn(flb_map* m, KnnArgs a) {
   return 0;
 }
 
-static int ensure_outbuf(flb_map* m, int n) {
-  if (n > m->outbuf_cap) {
-    if (m->outbuf) cudaFree(m->outbuf);
-    m->outbuf = nullptr; m->outbuf_cap = 0;
-    int cap = std::max(n, 1 << 16);
-    CU(cudaMalloc((void**)&m->outbuf, sizeof(float4) * (size_t)cap));
-    m->outbuf_cap = cap;
-  }
-  return 0;
-}
+static int ensure_outbuf(flb_map* m, int n) { return grow(m->outbuf, sizeof(float4) * (size_t)n, sizeof(float4) << 16); }
 
 static int nearest_search_impl(flb_map* m, const float* q_xyz, int nq, int stride, int k, float max_dist, float* out_pts, int out_w,
                                float* out_d2, int* out_cnt) {
@@ -572,7 +587,7 @@ static int nearest_search_impl(flb_map* m, const float* q_xyz, int nq, int strid
   float* dint = nullptr;
   CU(cudaMalloc((void**)&dcnt, nq));
   KnnArgs a;
-  a.m = m->d; a.q = m->stage; a.n = nq; a.nbr = m->outbuf; a.cnt = dcnt;
+  a.m = m->d; a.q = m->stage.p; a.n = nq; a.nbr = m->outbuf.p; a.cnt = dcnt;
   a.max_d2 = (max_dist > 0.f && max_dist < 1e18f) ? max_dist * max_dist : INFINITY;
   a.phase_stats = nullptr;
   a.ctl = nullptr; a.body = nullptr; a.stride = nq; a.work_count = nullptr;
@@ -586,12 +601,12 @@ static int nearest_search_impl(flb_map* m, const float* q_xyz, int nq, int strid
     hi.resize((size_t)nq * K);
     le = cudaMalloc((void**)&dint, sizeof(float) * hi.size());
     if (le == cudaSuccess) {
-      k_lookup_intensity<<<grid_for(nq * K, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->d, m->outbuf, dint, nq * K);
+      k_lookup_intensity<<<grid_for(nq * K, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->d, m->outbuf.p, dint, nq * K);
       m->launches++;
       le = cudaMemcpyAsync(hi.data(), dint, sizeof(float) * hi.size(), cudaMemcpyDeviceToHost, m->stream);
     }
   }
-  if (le == cudaSuccess) le = cudaMemcpyAsync(h.data(), m->outbuf, sizeof(float4) * h.size(), cudaMemcpyDeviceToHost, m->stream);
+  if (le == cudaSuccess) le = cudaMemcpyAsync(h.data(), m->outbuf.p, sizeof(float4) * h.size(), cudaMemcpyDeviceToHost, m->stream);
   if (le == cudaSuccess) le = cudaMemcpyAsync(hc.data(), dcnt, nq, cudaMemcpyDeviceToHost, m->stream);
   if (le == cudaSuccess) le = cudaStreamSynchronize(m->stream);
   cudaFree(dcnt);
@@ -635,7 +650,7 @@ static int collect_common(flb_map* m, int mode, const float* params, int nparams
   if (cap > 0 && ensure_outbuf(m, cap)) return 1;
   if (nparams && upload_params(m, params, nparams)) return 1;
   CU(cudaMemsetAsync(m->d_misc, 0, sizeof(int), m->stream));
-  k_collect<<<grid_for(nblk * 32, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->d, nblk, mode, m->dparams, cap ? m->outbuf : nullptr, cap, m->d_misc);
+  k_collect<<<grid_for(nblk * 32, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->d, nblk, mode, m->dparams.p, cap ? m->outbuf.p : nullptr, cap, m->d_misc);
   m->launches++;
   CU(cudaGetLastError());
   int total = 0;
@@ -645,7 +660,7 @@ static int collect_common(flb_map* m, int mode, const float* params, int nparams
   const int w = std::min(total, cap);
   if (w > 0) {
     std::vector<float4> h(w);
-    CU(cudaMemcpy(h.data(), m->outbuf, sizeof(float4) * w, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(h.data(), m->outbuf.p, sizeof(float4) * w, cudaMemcpyDeviceToHost));
     if (out_w == 4) memcpy(out_xyz, h.data(), sizeof(float4) * (size_t)w);
     else for (int i = 0; i < w; ++i) { out_xyz[3 * i] = h[i].x; out_xyz[3 * i + 1] = h[i].y; out_xyz[3 * i + 2] = h[i].z; }
   }
@@ -764,18 +779,12 @@ extern "C" int flb_debug_knn_bench(flb_map* m, const float* q_xyz, int nq, int s
   CU(cudaSetDevice(m->cfg.device));
   if (upload_points(m, q_xyz, nq, stride)) return 1;
   if (ensure_outbuf(m, nq * 5)) return 1;
-  if (nq > m->work_cap) {
-    if (m->worklist) cudaFree(m->worklist);
-    m->worklist = nullptr; m->work_cap = 0;
-    CU(cudaMalloc((void**)&m->worklist, sizeof(int) * (size_t)std::max(nq, 1 << 17)));
-    m->work_cap = std::max(nq, 1 << 17);
-    m->gen++;
-  }
+  if (ensure_worklist(m, nq)) return 1;
   unsigned char* dcnt = nullptr;
   CU(cudaMalloc((void**)&dcnt, nq));
   KnnArgs a;
-  a.m = m->d; a.q = m->stage; a.n = nq; a.nbr = m->outbuf; a.cnt = dcnt; a.max_d2 = INFINITY; a.phase_stats = nullptr;
-  a.worklist = m->worklist; a.work_count = m->d_misc + 12; a.work_ticket = m->d_misc + 13; a.ctl = nullptr; a.body = nullptr; a.stride = nq;
+  a.m = m->d; a.q = m->stage.p; a.n = nq; a.nbr = m->outbuf.p; a.cnt = dcnt; a.max_d2 = INFINITY; a.phase_stats = nullptr;
+  a.worklist = m->worklist.p; a.work_count = m->d_misc + 12; a.work_ticket = m->d_misc + 13; a.ctl = nullptr; a.body = nullptr; a.stride = nq;
   cudaError_t e = cudaFuncSetAttribute(k_knn_tile<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (e == cudaSuccess) e = cudaEventCreate(&e0);
@@ -796,7 +805,7 @@ extern "C" int flb_debug_knn_bench(flb_map* m, const float* q_xyz, int nq, int s
   if (e == cudaSuccess && unresolved) e = cudaMemcpy(unresolved, a.work_count, sizeof(int), cudaMemcpyDeviceToHost);
   if (e == cudaSuccess && out_d2) {
     std::vector<float4> h((size_t)nq * 5);
-    e = cudaMemcpy(h.data(), m->outbuf, sizeof(float4) * h.size(), cudaMemcpyDeviceToHost);
+    e = cudaMemcpy(h.data(), m->outbuf.p, sizeof(float4) * h.size(), cudaMemcpyDeviceToHost);
     for (int i = 0; i < nq && e == cudaSuccess; ++i)
       for (int j = 0; j < 5; ++j) out_d2[(size_t)i * 5 + j] = h[(size_t)j * nq + i].w;
   }
@@ -825,31 +834,22 @@ struct flb_session {
   int* selint = nullptr;
   void* cub_tmp = nullptr;
   size_t cub_tmp_bytes = 0;
-  double* drows = nullptr;  // M x 13 export buffer
-  int drows_cap = 0;
+  DevBuf<double> drows;     // M x 13 export buffer, column-major, leading dimension = its row capacity (drows_ld)
   double* h_out = nullptr;  // pinned NACC
   int* h_cnt2 = nullptr;    // pinned 4 ints
   int* d_cnt2 = nullptr;
   int res_grid = 0;
   PoseDev last_pose{};
   bool have_pass = false;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
-  unsigned char* raw = nullptr;
-  size_t raw_cap = 0;
+  DevBuf<unsigned char> raw;     // staging of strided scan records
   // device-driven update
   EsikfCtl* ctl = nullptr;       // device
   EsikfCtl* h_ctl = nullptr;     // pinned scratch (initial upload of ctl)
-  double* h_x0P0 = nullptr;      // working: MAPPED pinned staging of a scan's inputs (k_esikf_begin reads it over PCIe)
-  double* d_x0P0 = nullptr;      //          its device-side address
-  StepResult* h_res = nullptr;   // working: MAPPED pinned result record written by k_publish
-  StepResult* d_res = nullptr;   //          its device-side address
   bool device_update = true;
   EsikfScratch* d_scr = nullptr;
   cudaStream_t side = nullptr;   // second stream: k_esikf_pre overlaps the measurement kernels of the same pass
   cudaEvent_t ev_fork[9] = {nullptr}, ev_join[9] = {nullptr};   // one pair per pass + [8] = the posterior's publish branch
-  cudaGraphExec_t graph[2] = {nullptr, nullptr};  // [0] update only, [1] update + map_incremental (no scan or host pointer baked in
-  int graph_kernels[2] = {0, 0};                  //  beyond the slot's own staging / result records)
-  int graph_gen = -1;            // flb_map::gen the graphs were captured at
+  int graph_gen = -1;            // flb_map::gen the graphs of both slots were captured at
   // FLB_HOST_TIMING=1: where the host side of a step goes (printed when the session is destroyed)
   bool host_timing = false;
   double ht_begin = 0, ht_launch = 0, ht_wait = 0, ht_finish = 0, ht_between = 0;
@@ -858,53 +858,31 @@ struct flb_session {
   bool use_graph = true;
   // double-buffered scan upload (flb_scan_prefetch)
   float4* body_alt = nullptr;
-  unsigned char* raw_alt = nullptr;
-  size_t raw_alt_cap = 0;
+  DevBuf<unsigned char> raw_alt; // staging of strided prefetched records (on copy_stream)
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_copy = nullptr;
   int pending_n = -1;            // >= 0: a prefetched scan waits in body_alt
-  // flb_scan_step_begin / _finish
-  bool step_pending = false, step_device = false, step_ev2 = false;
   bool flags_clean = false;      // sel / cnt hold their per-scan initial values (see scan_reset)
-  int step_l0 = 0, step_deleted = 0, step_flg = 1, step_n = 0;
-  double step_x[26], step_P[NDOF * NDOF];
   // Up to TWO steps may be in flight (begin, begin, finish, begin, finish, ...): everything of a step that lives on the host —
-  // pinned input / result buffers, the graphs whose copy nodes point at them, timing events, the bookkeeping above — exists
-  // once per slot; the members above are the WORKING set = a copy of slot[active] (use_slot switches).  Device buffers are
-  // shared: the steps execute one after the other on the map's stream.
+  // pinned input / result records, the graphs whose copy nodes point at them, timing events, the step's bookkeeping —
+  // exists once per slot, and every call works on slot[active] (cur).  Device buffers are shared: the steps execute one
+  // after the other on the map's stream.
   struct StepSlot {
-    double *h_x0P0 = nullptr, *d_x0P0 = nullptr;
-    StepResult *h_res = nullptr, *d_res = nullptr;
-    cudaGraphExec_t graph[2] = {nullptr, nullptr};
-    int gk[2] = {0, 0};
+    double *h_x0P0 = nullptr, *d_x0P0 = nullptr;     // MAPPED pinned staging of a scan's inputs (k_esikf_begin reads it over
+                                                     // PCIe), its device-side address
+    StepResult *h_res = nullptr, *d_res = nullptr;   // MAPPED pinned result record written by k_publish, its device address
+    cudaGraphExec_t graph[2] = {nullptr, nullptr};   // [0] update only, [1] update + map_incremental (no scan or host pointer
+    int graph_kernels[2] = {0, 0};                   //  baked in beyond this slot's own staging / result records)
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
-    bool pending = false, device = false, ev2_on = false;
+    // flb_scan_step_begin / _finish
+    bool device = false, ev2_on = false;
     int l0 = 0, deleted = 0, flg = 1, n = 0;
     double x[26], P[NDOF * NDOF];
   } slot[2];
   int active = 0, head = 0, npending = 0;
 };
 
-// working set <-> slots
-static void save_active(flb_session* s) {
-  flb_session::StepSlot& o = s->slot[s->active];
-  for (int i = 0; i < 2; ++i) { o.graph[i] = s->graph[i]; o.gk[i] = s->graph_kernels[i]; }
-  o.pending = s->step_pending; o.device = s->step_device; o.ev2_on = s->step_ev2; o.l0 = s->step_l0; o.deleted = s->step_deleted; o.flg = s->step_flg; o.n = s->step_n;
-  memcpy(o.x, s->step_x, sizeof(o.x));
-  memcpy(o.P, s->step_P, sizeof(o.P));
-}
-static void use_slot(flb_session* s, int j) {
-  if (j == s->active) return;
-  save_active(s);
-  const flb_session::StepSlot& w = s->slot[j];
-  s->h_x0P0 = w.h_x0P0; s->d_x0P0 = w.d_x0P0; s->h_res = w.h_res; s->d_res = w.d_res;
-  for (int i = 0; i < 2; ++i) { s->graph[i] = w.graph[i]; s->graph_kernels[i] = w.gk[i]; }
-  s->ev0 = w.ev0; s->ev1 = w.ev1; s->ev2 = w.ev2; s->ev3 = w.ev3;
-  s->step_pending = w.pending; s->step_device = w.device; s->step_ev2 = w.ev2_on; s->step_l0 = w.l0; s->step_deleted = w.deleted; s->step_flg = w.flg; s->step_n = w.n;
-  memcpy(s->step_x, w.x, sizeof(w.x));
-  memcpy(s->step_P, w.P, sizeof(w.P));
-  s->active = j;
-}
+static inline flb_session::StepSlot& cur(flb_session* s) { return s->slot[s->active]; }
 
 extern "C" void flb_session_default_config(flb_session_config* c) {
   if (!c) return;
@@ -964,10 +942,6 @@ extern "C" int flb_session_create(flb_map* m, const flb_session_config* cfg, flb
   }
   if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_out, sizeof(double) * NACC);
   if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_cnt2, sizeof(int) * 8);
-  if (e == cudaSuccess) e = cudaEventCreate(&s->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&s->ev1);
-  if (e == cudaSuccess) e = cudaEventCreate(&s->ev2);
-  if (e == cudaSuccess) e = cudaEventCreate(&s->ev3);
   if (e == cudaSuccess) {
     size_t tb = 0;
     e = cub::DeviceScan::ExclusiveSum(nullptr, tb, s->selint, s->offs, s->cap, m->stream);
@@ -990,15 +964,11 @@ extern "C" int flb_session_create(flb_map* m, const flb_session_config* cfg, flb
     if (e == cudaSuccess) e = cudaHostAlloc((void**)&w.h_res, sizeof(StepResult), cudaHostAllocMapped);
     if (e == cudaSuccess) e = cudaHostGetDevicePointer((void**)&w.d_res, w.h_res, 0);
     if (e == cudaSuccess) { memset(w.h_x0P0, 0, sizeof(double) * (26 + NDOF * NDOF + 4)); memset(w.h_res, 0, sizeof(StepResult)); }
-    if (j == 0) { w.ev0 = s->ev0; w.ev1 = s->ev1; w.ev2 = s->ev2; w.ev3 = s->ev3; }
-    else {
-      if (e == cudaSuccess) e = cudaEventCreate(&w.ev0);
-      if (e == cudaSuccess) e = cudaEventCreate(&w.ev1);
-      if (e == cudaSuccess) e = cudaEventCreate(&w.ev2);
-      if (e == cudaSuccess) e = cudaEventCreate(&w.ev3);
-    }
+    if (e == cudaSuccess) e = cudaEventCreate(&w.ev0);
+    if (e == cudaSuccess) e = cudaEventCreate(&w.ev1);
+    if (e == cudaSuccess) e = cudaEventCreate(&w.ev2);
+    if (e == cudaSuccess) e = cudaEventCreate(&w.ev3);
   }
-  if (e == cudaSuccess) { s->h_x0P0 = s->slot[0].h_x0P0; s->d_x0P0 = s->slot[0].d_x0P0; s->h_res = s->slot[0].h_res; s->d_res = s->slot[0].d_res; }
   s->body_cur = s->body;
   if (e != cudaSuccess) { flb_session_destroy(s); return set_err("flb_session_create: %s", cudaGetErrorString(e)); }
   if (const char* ht = getenv("FLB_HOST_TIMING")) s->host_timing = atoi(ht) != 0;
@@ -1016,24 +986,18 @@ extern "C" void flb_session_destroy(flb_session* s) {
   Q(cudaStreamSynchronize(s->map->stream));
   if (s->side) Q(cudaStreamSynchronize(s->side));
   if (s->copy_stream) Q(cudaStreamSynchronize(s->copy_stream));
-  save_active(s);
-  for (int j = 0; j < 2; ++j)
-    for (int i = 0; i < 2; ++i)
-      if (s->slot[j].graph[i]) Q(cudaGraphExecDestroy(s->slot[j].graph[i]));
+  for (const flb_session::StepSlot& w : s->slot) {
+    for (cudaGraphExec_t g : w.graph) if (g) Q(cudaGraphExecDestroy(g));
+    if (w.h_x0P0) Q(cudaFreeHost(w.h_x0P0));
+    if (w.h_res) Q(cudaFreeHost(w.h_res));
+    for (cudaEvent_t e : {w.ev0, w.ev1, w.ev2, w.ev3}) if (e) Q(cudaEventDestroy(e));
+  }
   void* ptrs[] = {s->body, s->body_alt, s->world, s->nbr, s->normvec, s->plane, s->cnt, s->sel, s->cls, s->partial, s->dout, s->offs, s->selint,
-                  s->cub_tmp, s->drows, s->d_cnt2, s->raw, s->raw_alt, s->ctl, s->d_scr};
+                  s->cub_tmp, s->d_cnt2, s->ctl, s->d_scr};
   for (void* p : ptrs) if (p) Q(cudaFree(p));
   if (s->h_out) Q(cudaFreeHost(s->h_out));
   if (s->h_cnt2) Q(cudaFreeHost(s->h_cnt2));
   if (s->h_ctl) Q(cudaFreeHost(s->h_ctl));
-  if (!s->slot[0].ev0) { s->slot[0].ev0 = s->ev0; s->slot[0].ev1 = s->ev1; s->slot[0].ev2 = s->ev2; s->slot[0].ev3 = s->ev3; }   // creation failed early
-  for (int j = 0; j < 2; ++j) {
-    flb_session::StepSlot& w = s->slot[j];
-    if (w.h_x0P0) Q(cudaFreeHost(w.h_x0P0));
-    if (w.h_res) Q(cudaFreeHost(w.h_res));
-    cudaEvent_t ev[] = {w.ev0, w.ev1, w.ev2, w.ev3};
-    for (cudaEvent_t e : ev) if (e) Q(cudaEventDestroy(e));
-  }
   if (s->ev_copy) Q(cudaEventDestroy(s->ev_copy));
   for (int i = 0; i < 9; ++i) {
     if (s->ev_fork[i]) Q(cudaEventDestroy(s->ev_fork[i]));
@@ -1084,24 +1048,9 @@ extern "C" int flb_scan_upload_pt(flb_session* s, const void* pts, int n, int st
   if (off_i >= 0 && off_i + 4 > stride) return set_err("intensity offset %d outside the %d-byte record", off_i, stride);
   CU(cudaSetDevice(s->map->cfg.device));
   flb_map* m = s->map;
-  if (n > 0) {
-    if (stride == 16 && (off_i < 0 || off_i == 12)) {
-      CU(cudaMemcpyAsync(s->body, pts, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, m->stream));
-    } else {
-      const size_t bytes = (size_t)(n - 1) * stride + (size_t)std::max(12, off_i + 4);
-      if (bytes > s->raw_cap) {
-        if (s->raw) cudaFree(s->raw);
-        s->raw = nullptr; s->raw_cap = 0;
-        const size_t rc = std::max(bytes, (size_t)s->cap * (size_t)stride);   // sized once for the session capacity
-        CU(cudaMalloc((void**)&s->raw, rc));
-        s->raw_cap = rc;
-      }
-      CU(cudaMemcpyAsync(s->raw, pts, bytes, cudaMemcpyHostToDevice, m->stream));
-      k_pack_points<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(s->raw, stride, off_i, s->body, n);
-      m->launches++;
-      CU(cudaGetLastError());
-    }
-  }
+  if (stride == 16 && off_i < 0) off_i = 12;
+  // (the staging is sized once for the session capacity)
+  if (n > 0 && upload_records(m, m->stream, s->raw, (size_t)s->cap * (size_t)stride, pts, n, stride, off_i, -1, s->body, nullptr)) return 1;
   return scan_reset(s, n);
 }
 // (the 4th float of a 16-byte record is carried as the point's intensity into the map; other strides: no intensity)
@@ -1114,22 +1063,10 @@ extern "C" int flb_scan_prefetch(flb_session* s, const float* xyz, int n, int st
   CU(cudaSetDevice(s->map->cfg.device));
   flb_map* m = s->map;
   if (n > 0) {
-    if (stride == 16) {
-      CU(cudaMemcpyAsync(s->body_alt, xyz, sizeof(float4) * (size_t)n, cudaMemcpyHostToDevice, s->copy_stream));
-    } else {
-      const size_t bytes = (size_t)n * 12;
-      if (bytes > s->raw_alt_cap) {
-        CU(cudaStreamSynchronize(s->copy_stream));
-        if (s->raw_alt) cudaFree(s->raw_alt);
-        s->raw_alt = nullptr; s->raw_alt_cap = 0;
-        CU(cudaMalloc((void**)&s->raw_alt, std::max(bytes, (size_t)1 << 20)));
-        s->raw_alt_cap = std::max(bytes, (size_t)1 << 20);
-      }
-      CU(cudaMemcpyAsync(s->raw_alt, xyz, bytes, cudaMemcpyHostToDevice, s->copy_stream));
-      k_pack_points<<<grid_for(n, 256, m->sm_count * 8), 256, 0, s->copy_stream>>>(s->raw_alt, 12, -1, s->body_alt, n);
-      m->launches++;
-      CU(cudaGetLastError());
-    }
+    // a 16-byte record carries its intensity, as for flb_scan_upload; the previous prefetch may still read raw_alt
+    if (stride == 12 && (size_t)n * 12 > s->raw_alt.cap) CU(cudaStreamSynchronize(s->copy_stream));
+    if (upload_records(m, s->copy_stream, s->raw_alt, (size_t)1 << 20, xyz, n, stride, stride == 16 ? 12 : -1, -1, s->body_alt, nullptr))
+      return 1;
   }
   CU(cudaEventRecord(s->ev_copy, s->copy_stream));
   s->pending_n = n;
@@ -1233,26 +1170,23 @@ extern "C" int flb_pass(flb_session* s, const double* state26, int search, flb_p
   return 0;
 }
 
+// rows the export buffer holds: the leading dimension of its columns
+static inline int drows_ld(const flb_session* s) { return (int)(s->drows.cap / (sizeof(double) * 13)); }
+
 // device export of rows in index order; returns M
 static int export_rows(flb_session* s, int M_expected) {
   flb_map* m = s->map;
   cudaStream_t st = m->stream;
   const int n = s->n;
-  if (M_expected > s->drows_cap) {
-    if (s->drows) cudaFree(s->drows);
-    s->drows = nullptr; s->drows_cap = 0;
-    int cap = std::max(M_expected, 1 << 14);
-    CU(cudaMalloc((void**)&s->drows, sizeof(double) * 13 * (size_t)cap));
-    s->drows_cap = cap;
-  }
+  if (grow(s->drows, sizeof(double) * 13 * (size_t)M_expected, sizeof(double) * 13 * ((size_t)1 << 14))) return 1;
   const int g = grid_for(n, 256, m->sm_count * 8);
   k_sel_to_int<<<g, 256, 0, st>>>(s->sel, s->selint, n);
   size_t tb = s->cub_tmp_bytes;
   CU(cub::DeviceScan::ExclusiveSum(s->cub_tmp, tb, s->selint, s->offs, n, st));
   const MeasArgs ma = meas_args(s, s->last_pose, 0);
-  const int ld = s->drows_cap;
-  if (s->cfg.extrinsic_est_en) k_rows<true><<<g, 256, 0, st>>>(ma, s->offs, s->drows, ld, s->drows + (size_t)12 * ld, s->drows_cap);
-  else k_rows<false><<<g, 256, 0, st>>>(ma, s->offs, s->drows, ld, s->drows + (size_t)12 * ld, s->drows_cap);
+  const int ld = drows_ld(s);
+  if (s->cfg.extrinsic_est_en) k_rows<true><<<g, 256, 0, st>>>(ma, s->offs, s->drows.p, ld, s->drows.p + (size_t)12 * ld, ld);
+  else k_rows<false><<<g, 256, 0, st>>>(ma, s->offs, s->drows.p, ld, s->drows.p + (size_t)12 * ld, ld);
   m->launches += 3;
   CU(cudaGetLastError());
   return 0;
@@ -1268,9 +1202,9 @@ extern "C" int flb_pass_rows(flb_session* s, double* hx, int ld, double* h, int 
   if (capacity_rows < Mexp || ld < Mexp) return set_err("flb_pass_rows: capacity %d / ld %d < M = %d", capacity_rows, ld, Mexp);
   if (export_rows(s, Mexp)) return 1;
   cudaStream_t st = s->map->stream;
-  const int dl = s->drows_cap;
-  if (hx) CU(cudaMemcpy2DAsync(hx, sizeof(double) * ld, s->drows, sizeof(double) * dl, sizeof(double) * Mexp, 12, cudaMemcpyDeviceToHost, st));
-  if (h) CU(cudaMemcpyAsync(h, s->drows + (size_t)12 * dl, sizeof(double) * Mexp, cudaMemcpyDeviceToHost, st));
+  const int dl = drows_ld(s);
+  if (hx) CU(cudaMemcpy2DAsync(hx, sizeof(double) * ld, s->drows.p, sizeof(double) * dl, sizeof(double) * Mexp, 12, cudaMemcpyDeviceToHost, st));
+  if (h) CU(cudaMemcpyAsync(h, s->drows.p + (size_t)12 * dl, sizeof(double) * Mexp, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return 0;
 }
@@ -1281,7 +1215,8 @@ static int run_update(flb_session* s, double* state26, double* P, flb_update_sta
   host::IteratedUpdate u(state26, P, s->cfg.laser_point_cov, s->cfg.max_iterations, s->cfg.limit);
   int passes = 0, searches = 0, lastM = 0;
   double lastres = 0;
-  CU(cudaEventRecord(s->ev0, m->stream));
+  const flb_session::StepSlot& w = cur(s);
+  CU(cudaEventRecord(w.ev0, m->stream));
   while (u.more()) {
     double cur[26];
     u.current_state(cur);
@@ -1303,21 +1238,21 @@ static int run_update(flb_session* s, double* state26, double* P, flb_update_sta
       const int M = r.effct_feat_num;
       if (export_rows(s, M)) return 1;
       std::vector<double> cm((size_t)13 * M), rows((size_t)12 * M), hv(M);
-      const int dl = s->drows_cap;
-      CU(cudaMemcpy2DAsync(cm.data(), sizeof(double) * M, s->drows, sizeof(double) * dl, sizeof(double) * M, 13, cudaMemcpyDeviceToHost, m->stream));
+      const int dl = drows_ld(s);
+      CU(cudaMemcpy2DAsync(cm.data(), sizeof(double) * M, s->drows.p, sizeof(double) * dl, sizeof(double) * M, 13, cudaMemcpyDeviceToHost, m->stream));
       CU(cudaStreamSynchronize(m->stream));
       for (int r_ = 0; r_ < M; ++r_) { for (int c = 0; c < 12; ++c) rows[(size_t)r_ * 12 + c] = cm[(size_t)c * M + r_]; hv[r_] = cm[(size_t)12 * M + r_]; }
       u.step_rows(rows.data(), hv.data(), M);
     }
   }
-  CU(cudaEventRecord(s->ev1, m->stream));
+  CU(cudaEventRecord(w.ev1, m->stream));
   u.result(state26, P);
   if (stats) {
     stats->passes = passes; stats->search_passes = searches; stats->effct_feat_num = lastM;
     stats->converged_count = u.converged_count(); stats->total_residual = lastres;
-    CU(cudaEventSynchronize(s->ev1));
+    CU(cudaEventSynchronize(w.ev1));
     float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, s->ev0, s->ev1));
+    CU(cudaEventElapsedTime(&ms, w.ev0, w.ev1));
     stats->gpu_ms = ms;
   }
   return 0;
@@ -1337,7 +1272,8 @@ static int enqueue_scan_device(flb_session* s, bool with_insert) {
   const bool overlap = !m->prof_on;  // per-class event timing needs a single in-order stream
   const bool md12 = s->cfg.extrinsic_est_en != 0;   // measured subspace: 12 columns with extrinsic estimation, else 6
   const int cap = s->cap;
-  launch_k(k_esikf_begin, 1, 256, 0, st, s->ctl, (const double*)s->d_x0P0, m->d_misc + 16);   // reads the mapped pinned staging record
+  const flb_session::StepSlot& w = cur(s);
+  launch_k(k_esikf_begin, 1, 256, 0, st, s->ctl, (const double*)w.d_x0P0, m->d_misc + 16);   // reads the mapped pinned staging record
   m->launches++;
   for (int p = 0; p <= s->cfg.max_iterations; ++p) {
     if (overlap) {
@@ -1349,9 +1285,9 @@ static int enqueue_scan_device(flb_session* s, bool with_insert) {
         // the insert's scratch hash and counters are cleared here, next to the first pass, instead of between the
         // insert kernels at the end of the scan (three memset nodes off the critical path)
         if (!m->capturing && ensure_scratch(m, cap)) return 1;
-        const uint32_t sc = next_pow2((uint64_t)std::max(cap, 512) * 2);
-        CU(cudaMemsetAsync(m->skeys, 0xFF, sizeof(uint64_t) * sc, s->side));
-        CU(cudaMemsetAsync(m->sbest, 0xFF, sizeof(unsigned long long) * sc, s->side));
+        const uint32_t sc = scratch_slots(cap);
+        CU(cudaMemsetAsync(m->skeys.p, 0xFF, sizeof(uint64_t) * sc, s->side));
+        CU(cudaMemsetAsync(m->sbest.p, 0xFF, sizeof(unsigned long long) * sc, s->side));
         CU(cudaMemsetAsync(s->d_cnt2, 0, sizeof(int) * 2, s->side));
         m->scratch_clean = true;
       }
@@ -1394,14 +1330,14 @@ static int enqueue_scan_device(flb_session* s, bool with_insert) {
   if (tail_publish) {
     CU(cudaEventRecord(s->ev_fork[8], st));
     CU(cudaStreamWaitEvent(s->side, s->ev_fork[8], 0));
-    k_publish<<<1, 256, 0, s->side>>>((const EsikfCtl*)s->ctl, nullptr, nullptr, s->d_res, 0);
+    k_publish<<<1, 256, 0, s->side>>>((const EsikfCtl*)s->ctl, nullptr, nullptr, w.d_res, 0);
     CU(cudaEventRecord(s->ev_join[8], s->side));
     m->launches++;
   }
   if (with_insert && enqueue_map_incremental(s, nullptr, 0, true, tail_publish)) return 1;
   if (tail_publish) CU(cudaStreamWaitEvent(st, s->ev_join[8], 0));
   else {
-    launch_k(k_publish, 1, 256, 0, st, (const EsikfCtl*)s->ctl, (const int*)m->d.counters, (const int*)(with_insert ? s->d_cnt2 : nullptr), s->d_res, 1);
+    launch_k(k_publish, 1, 256, 0, st, (const EsikfCtl*)s->ctl, (const int*)m->d.counters, (const int*)(with_insert ? s->d_cnt2 : nullptr), w.d_res, 1);
     m->launches++;
   }
   CU(cudaGetLastError());
@@ -1412,35 +1348,28 @@ static int enqueue_scan_device(flb_session* s, bool with_insert) {
 // Stage a scan's inputs and run the device-driven sequence, through a CUDA graph when possible.
 static int launch_scan_device(flb_session* s, const double* state26, const double* P, int flg_EKF_inited, bool with_insert) {
   flb_map* m = s->map;
-  memcpy(s->h_x0P0, state26, sizeof(double) * 26);
-  memcpy(s->h_x0P0 + 26, P, sizeof(double) * NDOF * NDOF);
-  s->h_x0P0[26 + NDOF * NDOF] = (double)s->n;
-  s->h_x0P0[26 + NDOF * NDOF + 1] = (double)flg_EKF_inited;
+  flb_session::StepSlot& w = cur(s);
+  double* x0P0 = w.h_x0P0;
+  memcpy(x0P0, state26, sizeof(double) * 26);
+  memcpy(x0P0 + 26, P, sizeof(double) * NDOF * NDOF);
+  x0P0[26 + NDOF * NDOF] = (double)s->n;
+  x0P0[26 + NDOF * NDOF + 1] = (double)flg_EKF_inited;
   {
     const unsigned long long bits = (unsigned long long)reinterpret_cast<uintptr_t>(s->body_cur);
-    memcpy(&s->h_x0P0[26 + NDOF * NDOF + 2], &bits, sizeof(bits));
+    memcpy(&x0P0[26 + NDOF * NDOF + 2], &bits, sizeof(bits));
   }
   const int gi = with_insert ? 1 : 0;
   if (!s->use_graph || m->prof_on) return enqueue_scan_device(s, with_insert);
   if (s->graph_gen != m->gen) {
     // a buffer baked into the captured sequences was reallocated (or the voxel size changed) since: capture again
-    flb_session::StepSlot& o = s->slot[1 - s->active];
-    for (int i = 0; i < 2; ++i) {
-      if (s->graph[i]) { Q(cudaGraphExecDestroy(s->graph[i])); s->graph[i] = nullptr; }
-      if (o.graph[i]) { Q(cudaGraphExecDestroy(o.graph[i])); o.graph[i] = nullptr; }
-    }
+    for (flb_session::StepSlot& o : s->slot)
+      for (cudaGraphExec_t& g : o.graph)
+        if (g) { Q(cudaGraphExecDestroy(g)); g = nullptr; }
     s->graph_gen = m->gen;   // (both slots start over: graphs are re-captured lazily, the first capture stamps this again)
   }
-  if (!s->graph[gi]) {
+  if (!w.graph[gi]) {
     // everything the captured sequence may allocate lazily must exist before capture
-    if (ensure_scratch(m, s->cap)) return 1;
-    if (s->cap > m->work_cap) {
-      if (m->worklist) cudaFree(m->worklist);
-      m->worklist = nullptr; m->work_cap = 0;
-      CU(cudaMalloc((void**)&m->worklist, sizeof(int) * (size_t)std::max(s->cap, 1 << 17)));
-      m->work_cap = std::max(s->cap, 1 << 17);
-      m->gen++;
-    }
+    if (ensure_scratch(m, s->cap) || ensure_worklist(m, s->cap)) return 1;
     CU(cudaStreamSynchronize(m->stream));
     const int l0 = m->launches;
     cudaGraph_t g = nullptr;
@@ -1456,19 +1385,19 @@ static int launch_scan_device(flb_session* s, const double* state26, const doubl
       m->launches = l0;
       return enqueue_scan_device(s, with_insert);
     }
-    ce = cudaGraphInstantiate(&s->graph[gi], g, 0);
+    ce = cudaGraphInstantiate(&w.graph[gi], g, 0);
     cudaGraphDestroy(g);
     if (ce != cudaSuccess) {
       cudaGetLastError();
-      s->graph[gi] = nullptr; s->use_graph = false; m->launches = l0;
+      w.graph[gi] = nullptr; s->use_graph = false; m->launches = l0;
       return enqueue_scan_device(s, with_insert);
     }
-    s->graph_kernels[gi] = m->launches - l0;
+    w.graph_kernels[gi] = m->launches - l0;
     m->launches = l0;
     s->graph_gen = m->gen;
   }
-  CU(cudaGraphLaunch(s->graph[gi], m->stream));
-  m->launches += s->graph_kernels[gi];
+  CU(cudaGraphLaunch(w.graph[gi], m->stream));
+  m->launches += w.graph_kernels[gi];
   return 0;
 }
 static int finish_counters(flb_map* m, const int* snapshot) {  // after the sequence completed: interpret the counters it copied
@@ -1490,16 +1419,17 @@ extern "C" int flb_esikf_update(flb_session* s, double* state26, double* P, flb_
   if (adopt_prefetched(s)) return 1;
   if (!s->device_update) return run_update(s, state26, P, stats);
   flb_map* m = s->map;
-  CU(cudaEventRecord(s->ev0, m->stream));
+  const flb_session::StepSlot& w = cur(s);
+  CU(cudaEventRecord(w.ev0, m->stream));
   if (launch_scan_device(s, state26, P, 1, false)) return 1;
-  CU(cudaEventRecord(s->ev1, m->stream));
+  CU(cudaEventRecord(w.ev1, m->stream));
   CU(cudaStreamSynchronize(m->stream));
-  if (finish_counters(m, s->h_res->counters)) return 1;
-  if (s->h_res->need_host) return run_update(s, state26, P, stats);  // M < 23: explicit-row branch on the host
-  memcpy(state26, s->h_res->x, sizeof(double) * 26);
-  memcpy(P, s->h_res->P, sizeof(double) * NDOF * NDOF);
-  stats_from_ctl(s->h_res, stats);
-  if (stats) CU(cudaEventElapsedTime(&stats->gpu_ms, s->ev0, s->ev1));
+  if (finish_counters(m, w.h_res->counters)) return 1;
+  if (w.h_res->need_host) return run_update(s, state26, P, stats);  // M < 23: explicit-row branch on the host
+  memcpy(state26, w.h_res->x, sizeof(double) * 26);
+  memcpy(P, w.h_res->P, sizeof(double) * NDOF * NDOF);
+  stats_from_ctl(w.h_res, stats);
+  if (stats) CU(cudaEventElapsedTime(&stats->gpu_ms, w.ev0, w.ev1));
   return 0;
 }
 
@@ -1510,20 +1440,19 @@ static int enqueue_map_incremental(flb_session* s, const double* state26, int fl
   if (n <= 0 && !from_ctl) return 0;
   const PoseDev pose = from_ctl ? PoseDev{} : pose_from(state26);
   const int npts = from_ctl ? s->cap : n;   // launch geometry / scratch size (the device count is read by the kernels)
+  const uint32_t sc = scratch_slots(npts);
   if (!m->scratch_clean) {
     // (inside the captured scan sequence these clears sit on the side branch of the first pass)
     if (!m->capturing && ensure_scratch(m, npts)) return 1;
-    const uint32_t sc0 = next_pow2((uint64_t)std::max(npts, 512) * 2);
     CU(cudaMemsetAsync(s->d_cnt2, 0, sizeof(int) * 2, st));
-    CU(cudaMemsetAsync(m->skeys, 0xFF, sizeof(uint64_t) * sc0, st));
-    CU(cudaMemsetAsync(m->sbest, 0xFF, sizeof(unsigned long long) * sc0, st));
+    CU(cudaMemsetAsync(m->skeys.p, 0xFF, sizeof(uint64_t) * sc, st));
+    CU(cudaMemsetAsync(m->sbest.p, 0xFF, sizeof(unsigned long long) * sc, st));
   }
-  const uint32_t sc = next_pow2((uint64_t)std::max(npts, 512) * 2);
   {
     ProfScope ps(m, FLB_K_CLASSIFY);
     launch_k(k_classify, grid_for(npts, 256, m->sm_count * 8), 256, 0, st, pose, (const EsikfCtl*)(from_ctl ? s->ctl : nullptr),
              (const float4*)s->body_cur, (const float4*)s->nbr, (const unsigned char*)s->cnt, n, s->cap, flg_EKF_inited, s->cfg.filter_size_map_min,
-             s->world, s->cls, s->d_cnt2, m->d, m->skeys, m->sbest, sc - 1);
+             s->world, s->cls, s->d_cnt2, m->d, m->skeys.p, m->sbest.p, sc - 1);
     m->launches++;
   }
   CU(cudaGetLastError());
@@ -1533,7 +1462,8 @@ static int enqueue_map_incremental(flb_session* s, const double* state26, int fl
       // the last block of the last insert kernel writes the map counters, map_incremental's counts and the step's device
       // span into the mapped pinned result record: no separate publishing kernel after the insert
       tail.ticket = s->d_cnt2 + 2; tail.counters = m->d.counters; tail.cnt2 = s->d_cnt2; tail.t_begin = &s->ctl->t_begin;
-      tail.out_counters = s->d_res->counters; tail.out_cnt2 = s->d_res->cnt2; tail.out_span = &s->d_res->span_ns;
+      StepResult* res = cur(s).d_res;
+      tail.out_counters = res->counters; tail.out_cnt2 = res->cnt2; tail.out_span = &res->span_ns;
     }
     if (insert_device(m, s->world, s->cls, s->cap, 2, &s->ctl->need_host, &s->ctl->n, true, tail)) return 1;
   } else if (insert_device(m, s->world, s->cls, n, 2, nullptr, nullptr, true)) return 1;
@@ -1658,35 +1588,35 @@ extern "C" int flb_scan_step_begin(flb_session* s, flb_fov_state* fov, const flo
   if (s->npending >= 2) return set_err("flb_scan_step_begin: two steps are already in flight (call flb_scan_step_finish first)");
   if (s->npending == 1 && !s->device_update)
     return set_err("flb_scan_step_begin: the host-driven engine runs one step at a time (call flb_scan_step_finish first)");
-  use_slot(s, (s->head + s->npending) & 1);
+  s->active = (s->head + s->npending) & 1;
+  flb_session::StepSlot& w = cur(s);
   const auto ht0 = std::chrono::steady_clock::now();
   if (s->host_timing && s->ht_n > 0) s->ht_between += std::chrono::duration<double>(ht0 - s->ht_last_finish).count();
   CU(cudaSetDevice(m->cfg.device));
-  s->step_l0 = m->launches;
-  s->step_deleted = 0;
-  s->step_flg = flg_EKF_inited;
-  memcpy(s->step_x, state26, sizeof(s->step_x));
-  memcpy(s->step_P, P, sizeof(s->step_P));
+  w.l0 = m->launches;
+  w.deleted = 0;
+  w.flg = flg_EKF_inited;
+  memcpy(w.x, state26, sizeof(w.x));
+  memcpy(w.P, P, sizeof(w.P));
   // A device-driven step without an on-stream upload times itself on the device (StepResult::span_ns): no event pair sits
   // on the stream between two steps in flight, only the one event flb_scan_step_finish waits on.
-  s->step_ev2 = body != nullptr || !s->device_update;
-  if (s->step_ev2) CU(cudaEventRecord(s->ev2, m->stream));
+  w.ev2_on = body != nullptr || !s->device_update;
+  if (w.ev2_on) CU(cudaEventRecord(w.ev2, m->stream));
   if (body) { if (flb_scan_upload(s, body, n, stride)) return 1; }
   else if (adopt_prefetched(s)) return 1;
   if (fov) {  // laserMapping.cpp:2320 (uses pos_lid of the previous posterior)
     int nb = 0;
-    if (flb_fov_segment(m, fov, fov->pos_lid, nullptr, &nb, &s->step_deleted)) return 1;
+    if (flb_fov_segment(m, fov, fov->pos_lid, nullptr, &nb, &w.deleted)) return 1;
   }
-  s->step_device = s->device_update;
-  if (s->step_device) {
+  w.device = s->device_update;
+  if (w.device) {
     const auto hl0 = std::chrono::steady_clock::now();
     if (launch_scan_device(s, state26, P, flg_EKF_inited, true)) return 1;  // :2380 + :2401, no host round trips inside
     if (s->host_timing) s->ht_launch += std::chrono::duration<double>(std::chrono::steady_clock::now() - hl0).count();
-    CU(cudaEventRecord(s->ev3, m->stream));
+    CU(cudaEventRecord(w.ev3, m->stream));
   }
-  s->step_n = s->n;
-  s->step_l0 = m->launches - s->step_l0;   // kernels launched by this step so far (a younger step may add its own before finish)
-  s->step_pending = true;
+  w.n = s->n;
+  w.l0 = m->launches - w.l0;   // kernels launched by this step so far (a younger step may add its own before finish)
   s->npending++;
   if (s->host_timing) s->ht_begin += std::chrono::duration<double>(std::chrono::steady_clock::now() - ht0).count();
   return 0;
@@ -1695,47 +1625,47 @@ extern "C" int flb_scan_step_begin(flb_session* s, flb_fov_state* fov, const flo
 extern "C" int flb_scan_step_finish(flb_session* s, flb_fov_state* fov, double* state26, double* P, flb_scan_result* out) {
   if (!s || !state26 || !P) return set_err("flb_scan_step: null argument");
   if (s->npending == 0) return set_err("flb_scan_step_finish without flb_scan_step_begin");
-  use_slot(s, s->head);          // the OLDEST step in flight
-  s->step_pending = false;
+  s->active = s->head;           // the OLDEST step in flight
+  const flb_session::StepSlot& w = cur(s);
   s->head ^= 1;
   s->npending--;
   flb_map* m = s->map;
   CU(cudaSetDevice(m->cfg.device));
   flb_scan_result r;
   memset(&r, 0, sizeof(r));
-  r.n_deleted = s->step_deleted;
-  bool host_path = !s->step_device;
+  r.n_deleted = w.deleted;
+  bool host_path = !w.device;
   float span_ms = 0.f;   // device-driven step: %globaltimer span of the whole sequence
   const int launches0 = m->launches;
   const auto hf0 = std::chrono::steady_clock::now();
   auto hf1 = hf0;
   if (!host_path) {
-    CU(cudaEventSynchronize(s->ev3));                      // the single synchronisation of the step (a younger step may be running on)
+    CU(cudaEventSynchronize(w.ev3));                      // the single synchronisation of the step (a younger step may be running on)
     hf1 = std::chrono::steady_clock::now();
-    if (finish_counters(m, s->h_res->counters)) return 1;
+    if (finish_counters(m, w.h_res->counters)) return 1;
     m->has_root = m->has_root || m->h_counters[CNT_VALID] > 0;
-    if (s->h_res->need_host) {
+    if (w.h_res->need_host) {
       if (s->npending)
         return set_err("flb_scan_step_finish: under-determined scan (fewer than 23 rows) while a younger step is already in flight; "
                        "such scans need the host-driven branch: run them with strictly alternating begin / finish");
       host_path = true;                                    // M < 23 branch: redo this scan on the host-driven path
     } else {
-      memcpy(state26, s->h_res->x, sizeof(double) * 26);
-      memcpy(P, s->h_res->P, sizeof(double) * NDOF * NDOF);
-      stats_from_ctl(s->h_res, &r.update);
-      s->h_cnt2[0] = s->h_res->cnt2[0];
-      s->h_cnt2[1] = s->h_res->cnt2[1];
-      r.update.gpu_ms = (float)((double)s->h_res->update_ns * 1e-6);
-      span_ms = (float)((double)s->h_res->span_ns * 1e-6);
+      memcpy(state26, w.h_res->x, sizeof(double) * 26);
+      memcpy(P, w.h_res->P, sizeof(double) * NDOF * NDOF);
+      stats_from_ctl(w.h_res, &r.update);
+      s->h_cnt2[0] = w.h_res->cnt2[0];
+      s->h_cnt2[1] = w.h_res->cnt2[1];
+      r.update.gpu_ms = (float)((double)w.h_res->update_ns * 1e-6);
+      span_ms = (float)((double)w.h_res->span_ns * 1e-6);
       if (r.update.gpu_ms > span_ms) r.update.gpu_ms = span_ms;   // (k_publish sits on a parallel branch: never report more than the whole)
     }
   }
   if (host_path) {
-    memcpy(state26, s->step_x, sizeof(s->step_x));
-    memcpy(P, s->step_P, sizeof(s->step_P));
+    memcpy(state26, w.x, sizeof(w.x));
+    memcpy(P, w.P, sizeof(w.P));
     if (run_update(s, state26, P, &r.update)) return 1;  // :2380
-    if (s->step_n > 0 && enqueue_map_incremental(s, state26, s->step_flg, false)) return 1;  // :2401
-    CU(cudaEventRecord(s->ev3, m->stream));
+    if (w.n > 0 && enqueue_map_incremental(s, state26, w.flg, false)) return 1;  // :2401
+    CU(cudaEventRecord(w.ev3, m->stream));
     if (fetch_counters(m)) return 1;
   }
   if (fov) {  // :2383 pos_lid = pos + rot * offset_T_L_I
@@ -1743,12 +1673,12 @@ extern "C" int flb_scan_step_finish(flb_session* s, flb_fov_state* fov, double* 
     host::V3 pl = x.pos + host::rotate(x.rot, x.offT);
     for (int i = 0; i < 3; ++i) fov->pos_lid[i] = pl.a[i];
   }
-  r.n_to_add = s->step_n > 0 ? s->h_cnt2[0] : 0;
-  r.n_no_downsample = s->step_n > 0 ? s->h_cnt2[1] : 0;
+  r.n_to_add = w.n > 0 ? s->h_cnt2[0] : 0;
+  r.n_no_downsample = w.n > 0 ? s->h_cnt2[1] : 0;
   r.map_valid = m->h_counters[CNT_VALID];
-  if (s->step_ev2) CU(cudaEventElapsedTime(&r.gpu_ms_total, s->ev2, s->ev3));
+  if (w.ev2_on) CU(cudaEventElapsedTime(&r.gpu_ms_total, w.ev2, w.ev3));
   else r.gpu_ms_total = span_ms > 0.f ? span_ms : r.update.gpu_ms;
-  r.kernel_launches = s->step_l0 + (m->launches - launches0);
+  r.kernel_launches = w.l0 + (m->launches - launches0);
   if (out) *out = r;
   const int rrc = maybe_rehash(m);
   if (s->host_timing) {

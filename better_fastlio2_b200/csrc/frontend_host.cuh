@@ -6,39 +6,30 @@
 
 // ------------------------------------------------------------------------------------------------ voxel-grid workspace
 struct VgWork {
-  int cap = 0;
-  unsigned *keys_a = nullptr, *keys_b = nullptr;
-  int *vals_a = nullptr, *vals_b = nullptr, *flags = nullptr, *pos = nullptr;
-  void* tmp = nullptr;
-  size_t tmp_bytes = 0;
-  unsigned* d_mm = nullptr;   // 8 words, see k_vg_init
-  unsigned* h_mm = nullptr;   // pinned mirror
+  int cap = 0;   // points the arrays and the CUB scratch are sized for
+  DevBuf<unsigned> keys_a, keys_b;
+  DevBuf<int> vals_a, vals_b, flags, pos;
+  DevBuf<unsigned char> tmp;   // CUB temporary storage
+  DevBuf<unsigned> d_mm;       // 8 words, see k_vg_init
+  PinnedBuf<unsigned> h_mm;    // pinned mirror
 };
-static void vg_release(VgWork& w) {
-  void* ptrs[] = {w.keys_a, w.keys_b, w.vals_a, w.vals_b, w.flags, w.pos, w.tmp, w.d_mm};
-  for (void* p : ptrs) if (p) Q(cudaFree(p));
-  if (w.h_mm) Q(cudaFreeHost(w.h_mm));
-  w = VgWork();
-}
 static int vg_ensure(VgWork& w, int n) {
   if (n <= w.cap) return 0;
-  vg_release(w);
+  w.cap = 0;   // (until every array has grown)
   const int cap = std::max(n, 1 << 12);
   size_t t1 = 0, t2 = 0;
   CU(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, cap));
   CU(cub::DeviceScan::ExclusiveSum(nullptr, t2, (const int*)nullptr, (int*)nullptr, cap));
-  w.tmp_bytes = std::max(t1, t2) + 256;
-  CU(cudaMalloc((void**)&w.keys_a, sizeof(unsigned) * (size_t)cap));
-  CU(cudaMalloc((void**)&w.keys_b, sizeof(unsigned) * (size_t)cap));
-  CU(cudaMalloc((void**)&w.vals_a, sizeof(int) * (size_t)cap));
-  CU(cudaMalloc((void**)&w.vals_b, sizeof(int) * (size_t)cap));
-  CU(cudaMalloc((void**)&w.flags, sizeof(int) * (size_t)cap));
-  CU(cudaMalloc((void**)&w.pos, sizeof(int) * (size_t)cap));
-  CU(cudaMalloc(&w.tmp, w.tmp_bytes));
-  CU(cudaMalloc((void**)&w.d_mm, sizeof(unsigned) * 8));
-  CU(cudaMallocHost((void**)&w.h_mm, sizeof(unsigned) * 8));
+  const size_t words = sizeof(unsigned) * (size_t)cap;
+  if (grow(w.keys_a, words, 0) || grow(w.keys_b, words, 0) || grow(w.vals_a, words, 0) || grow(w.vals_b, words, 0) ||
+      grow(w.flags, words, 0) || grow(w.pos, words, 0) || grow(w.tmp, std::max(t1, t2) + 256, 0) ||
+      grow(w.d_mm, sizeof(unsigned) * 8, 0) || grow(w.h_mm, sizeof(unsigned) * 8, 0))
+    return 1;
   w.cap = cap;
   return 0;
+}
+static size_t vg_device_bytes(const VgWork& w) {
+  return w.keys_a.cap + w.keys_b.cap + w.vals_a.cap + w.vals_b.cap + w.flags.cap + w.pos.cap + w.tmp.cap + w.d_mm.cap;
 }
 
 // pcl::VoxelGrid::applyFilter on n device points (x,y,z,intensity [+curvature]) -> out (capacity out_cap points), all on
@@ -46,23 +37,24 @@ static int vg_ensure(VgWork& w, int n) {
 static int vg_enqueue(flb_map* m, VgWork& w, const float4* pts, const float* curv, int n, float leaf, float4* out, float* out_curv,
                       int out_cap, cudaStream_t st) {
   if (vg_ensure(w, n)) return 1;
+  unsigned* mm = w.d_mm.p;
   const float inv = 1.0f / leaf;   // inverse_leaf_size_
   const int g = grid_for(std::max(n, 1), 256, m->sm_count * 8);
-  k_vg_init<<<1, 32, 0, st>>>(w.d_mm);
+  k_vg_init<<<1, 32, 0, st>>>(mm);
   m->launches++;
   if (n > 0) {
-    k_vg_minmax<<<g, 256, 0, st>>>(pts, n, w.d_mm);
-    k_vg_keys<<<g, 256, 0, st>>>(pts, n, inv, w.d_mm, w.keys_a, w.vals_a);
-    size_t tb = w.tmp_bytes;
-    CU(cub::DeviceRadixSort::SortPairs(w.tmp, tb, (const unsigned*)w.keys_a, w.keys_b, (const int*)w.vals_a, w.vals_b, n, 0, 32, st));
-    k_vg_heads<<<g, 256, 0, st>>>(w.keys_b, n, w.flags);
-    tb = w.tmp_bytes;
-    CU(cub::DeviceScan::ExclusiveSum(w.tmp, tb, (const int*)w.flags, w.pos, n, st));
-    k_vg_centroid<<<g, 256, 0, st>>>(pts, curv, w.keys_b, w.vals_b, w.flags, w.pos, n, out, out_curv, out_cap, w.d_mm);
+    k_vg_minmax<<<g, 256, 0, st>>>(pts, n, mm);
+    k_vg_keys<<<g, 256, 0, st>>>(pts, n, inv, mm, w.keys_a.p, w.vals_a.p);
+    size_t tb = w.tmp.cap;
+    CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)w.keys_a.p, w.keys_b.p, (const int*)w.vals_a.p, w.vals_b.p, n, 0, 32, st));
+    k_vg_heads<<<g, 256, 0, st>>>(w.keys_b.p, n, w.flags.p);
+    tb = w.tmp.cap;
+    CU(cub::DeviceScan::ExclusiveSum(w.tmp.p, tb, (const int*)w.flags.p, w.pos.p, n, st));
+    k_vg_centroid<<<g, 256, 0, st>>>(pts, curv, w.keys_b.p, w.vals_b.p, w.flags.p, w.pos.p, n, out, out_curv, out_cap, mm);
     m->launches += 4 + 6;   // + the radix-sort (histogram, 4 onesweep passes) and scan kernels of CUB
   }
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(w.h_mm, w.d_mm, sizeof(unsigned) * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(w.h_mm.p, mm, sizeof(unsigned) * 8, cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
@@ -75,8 +67,7 @@ struct flb_frontend {
   int n_raw = 0;            // points of the current raw scan (meas.lidar)
   int n_down = -1;          // points of feats_down_body after the last voxel filter (-1: none yet)
   bool sorted = false;      // pts_t holds feats_undistort (time order); else `pts` (upload order) is current
-  unsigned char* raw = nullptr;
-  size_t raw_cap = 0;
+  DevBuf<unsigned char> raw;   // staging of host records
   float4 *pts = nullptr, *pts_t = nullptr;
   float *curv = nullptr, *curv_t = nullptr, *down_curv = nullptr;
   int* perm = nullptr;      // time-sorted position -> upload index
@@ -125,12 +116,11 @@ extern "C" void flb_frontend_destroy(flb_frontend* f) {
   if (!f) return;
   flb_map* m = f->ses ? f->ses->map : nullptr;
   if (m) { Q(cudaSetDevice(m->cfg.device)); Q(cudaStreamSynchronize(m->stream)); }
-  void* ptrs[] = {f->raw, f->pts, f->pts_t, f->world, f->curv, f->curv_t, f->down_curv, f->perm, f->d_poses};
+  void* ptrs[] = {f->pts, f->pts_t, f->world, f->curv, f->curv_t, f->down_curv, f->perm, f->d_poses};
   for (void* p : ptrs) if (p) Q(cudaFree(p));
   if (f->h_poses) Q(cudaFreeHost(f->h_poses));
   if (f->ev_poses) Q(cudaEventDestroy(f->ev_poses));
   const bool counted = f->holds_ref;
-  vg_release(f->vg);
   pp_release(f->pp);
   delete f;
   if (m && counted) map_release(m);
@@ -138,20 +128,6 @@ extern "C" void flb_frontend_destroy(flb_frontend* f) {
 
 static inline const float4* fe_cloud(const flb_frontend* f) { return f->sorted ? f->pts_t : f->pts; }
 static inline const float* fe_curv(const flb_frontend* f) { return f->sorted ? f->curv_t : f->curv; }
-
-// copy n host records of `stride` bytes into the front end's raw staging buffer (on the session stream)
-static int fe_stage_raw(flb_frontend* f, flb_map* m, const void* src, int n, int stride) {
-  const size_t bytes = (size_t)n * stride;
-  if (bytes > f->raw_cap) {
-    if (f->raw) cudaFree(f->raw);
-    f->raw = nullptr; f->raw_cap = 0;
-    const size_t cap = std::max(bytes, (size_t)f->cap * (size_t)stride);   // sized once for the capacity: scans vary in size
-    CU(cudaMalloc((void**)&f->raw, cap));
-    f->raw_cap = cap;
-  }
-  CU(cudaMemcpyAsync(f->raw, src, bytes, cudaMemcpyHostToDevice, m->stream));
-  return 0;
-}
 
 extern "C" int flb_frontend_upload(flb_frontend* f, const void* pts, int n, int stride, int off_intensity, int off_curvature) {
   if (!f) return set_err("null front end");
@@ -165,11 +141,8 @@ extern "C" int flb_frontend_upload(flb_frontend* f, const void* pts, int n, int 
   f->sorted = false;
   f->n_down = -1;
   if (n == 0) return 0;
-  if (fe_stage_raw(f, m, pts, n, stride)) return 1;
-  k_pack_xyzic<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(f->raw, stride, off_intensity, off_curvature, f->pts, f->curv, n);
-  m->launches++;
-  CU(cudaGetLastError());
-  return 0;
+  // the staging is sized once for the capacity (scans vary in size); with the curvature always written, every stride packs
+  return upload_records(m, m->stream, f->raw, (size_t)f->cap * (size_t)stride, pts, n, stride, off_intensity, off_curvature, f->pts, f->curv);
 }
 
 extern "C" int flb_frontend_undistort(flb_frontend* f, const double* imu_poses22, int n_poses, const double* state26_end) {
@@ -188,9 +161,10 @@ extern "C" int flb_frontend_undistort(flb_frontend* f, const double* imu_poses22
   CU(cudaEventRecord(f->ev_poses, st));
   const int g = grid_for(n, 256, m->sm_count * 8);
   // sort(pcl_out.points.begin(), pcl_out.points.end(), time_list)  (IMU_Processing.hpp:243) — stable here
-  k_time_keys<<<g, 256, 0, st>>>(f->curv, f->vg.keys_a, f->vg.vals_a, n);
-  size_t tb = f->vg.tmp_bytes;
-  CU(cub::DeviceRadixSort::SortPairs(f->vg.tmp, tb, (const unsigned*)f->vg.keys_a, f->vg.keys_b, (const int*)f->vg.vals_a, f->perm, n, 0, 32, st));
+  VgWork& v = f->vg;
+  k_time_keys<<<g, 256, 0, st>>>(f->curv, v.keys_a.p, v.vals_a.p, n);
+  size_t tb = v.tmp.cap;
+  CU(cub::DeviceRadixSort::SortPairs(v.tmp.p, tb, (const unsigned*)v.keys_a.p, v.keys_b.p, (const int*)v.vals_a.p, f->perm, n, 0, 32, st));
   UndistortEnd e;
   for (int k = 0; k < 4; ++k) { e.rot[k] = state26_end[3 + k]; e.offR[k] = state26_end[7 + k]; }
   for (int k = 0; k < 3; ++k) { e.pos[k] = state26_end[k]; e.offT[k] = state26_end[11 + k]; }
@@ -213,8 +187,8 @@ extern "C" int flb_frontend_voxel_filter(flb_frontend* f, float leaf, int* n_out
   // the centroids are written straight into the session's feats_down_body buffer
   if (vg_enqueue(m, f->vg, fe_cloud(f), fe_curv(f), n, leaf, s->body, f->down_curv, s->cap, m->stream)) return 1;
   CU(cudaStreamSynchronize(m->stream));
-  int nd = (int)f->vg.h_mm[7];
-  if (f->vg.h_mm[6]) {
+  int nd = (int)f->vg.h_mm.p[7];
+  if (f->vg.h_mm.p[6]) {
     // PCL: "Leaf size is too small for the input dataset. Integer indices would overflow." -> output = input
     if (n > s->cap) return set_err("voxel filter overflow guard: unfiltered scan of %d points exceeds max_scan_points=%d", n, s->cap);
     CU(cudaMemcpyAsync(s->body, fe_cloud(f), sizeof(float4) * (size_t)n, cudaMemcpyDeviceToDevice, m->stream));
@@ -292,16 +266,6 @@ extern "C" int flb_frontend_points_to_world(flb_frontend* f, int which, const do
 }
 
 // ------------------------------------------------------------------------------------------------ stand-alone filters
-static int upload_xyzi(flb_map* m, const void* pts, int n, int stride, int off_intensity, unsigned char** raw, float4* dst) {
-  const size_t bytes = (size_t)n * stride;
-  CU(cudaMalloc((void**)raw, bytes));
-  CU(cudaMemcpyAsync(*raw, pts, bytes, cudaMemcpyHostToDevice, m->stream));
-  k_pack_xyzic<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(*raw, stride, off_intensity, -1, dst, nullptr, n);
-  m->launches++;
-  CU(cudaGetLastError());
-  return 0;
-}
-
 extern "C" int flb_voxel_grid_filter(flb_map* m, const void* pts, int n, int stride, int off_intensity, float leaf, float* out_xyzi,
                                      int cap, int* n_out) {
   if (!m) return set_err("null map");
@@ -312,27 +276,25 @@ extern "C" int flb_voxel_grid_filter(flb_map* m, const void* pts, int n, int str
   if (!pts || stride < 12) return set_err("bad point buffer");
   if (off_intensity >= 0 && off_intensity + 4 > stride) return set_err("field offset outside the point stride");
   CU(cudaSetDevice(m->cfg.device));
-  VgWork w;
-  unsigned char* raw = nullptr;
+  VgWork w;                     // per-call workspace and staging, freed on return
+  DevBuf<unsigned char> raw;
   float4 *in = nullptr, *out = nullptr;
   int rc = 0;
   auto body = [&]() -> int {
     CU(cudaMalloc((void**)&in, sizeof(float4) * (size_t)n));
     CU(cudaMalloc((void**)&out, sizeof(float4) * (size_t)n));
-    if (upload_xyzi(m, pts, n, stride, off_intensity, &raw, in)) return 1;
+    if (upload_records(m, m->stream, raw, 0, pts, n, stride, off_intensity, -1, in, nullptr)) return 1;
     if (vg_enqueue(m, w, in, nullptr, n, leaf, out, nullptr, n, m->stream)) return 1;
     CU(cudaStreamSynchronize(m->stream));
-    const bool ovf = w.h_mm[6] != 0;
-    const int nd = ovf ? n : (int)w.h_mm[7];
+    const bool ovf = w.h_mm.p[6] != 0;
+    const int nd = ovf ? n : (int)w.h_mm.p[7];
     if (n_out) *n_out = nd;
     const int c = std::min(nd, cap);
     if (c > 0 && out_xyzi) CU(cudaMemcpy(out_xyzi, ovf ? in : out, sizeof(float4) * (size_t)c, cudaMemcpyDeviceToHost));
     return 0;
   };
   rc = body();
-  if (raw) Q(cudaFree(raw));
   if (in) Q(cudaFree(in));
   if (out) Q(cudaFree(out));
-  vg_release(w);
   return rc;
 }

@@ -14,38 +14,25 @@
 // flb_map_release_keyframe_scratch frees it (e.g. after saving a map of the whole run).
 struct KfWork {
   VgWork vg;                                   // voxel grid of the sub-map / saved map
-  float *cin = nullptr, *cout = nullptr;       // curvature of an assembly and of its filtered output
-  size_t cin_cap = 0, cout_cap = 0;            // bytes
-  KfSeg *d_seg = nullptr, *h_seg = nullptr;    // segment table of k_kf_assemble (device, pinned staging)
-  int seg_cap = 0;
+  DevBuf<float> cin, cout;                     // curvature of an assembly and of its filtered output
+  DevBuf<KfSeg> d_seg;                         // segment table of k_kf_assemble
+  PinnedBuf<KfSeg> h_seg;                      //   and its staging
   cudaEvent_t ev_seg = nullptr;                // the last copy out of h_seg
-  ScChunk *d_chunk = nullptr, *h_chunk = nullptr;   // chunk table of k_sc_bins (device, pinned staging)
-  int chunk_cap = 0;
-  unsigned *d_sc_keys = nullptr, *h_sc_keys = nullptr;   // Scan Context keys, SC_BINS per descriptor (device, pinned)
-  int sc_cap = 0;                              // descriptors
+  DevBuf<ScChunk> d_chunk;                     // chunk table of k_sc_bins
+  PinnedBuf<ScChunk> h_chunk;                  //   and its staging
+  DevBuf<unsigned> d_sc_keys;                  // Scan Context keys, SC_BINS per descriptor
+  PinnedBuf<unsigned> h_sc_keys;               //   and their staging
 };
 
 static void kfw_release(KfWork* w) {
   if (!w) return;
-  vg_release(w->vg);
-  void* ptrs[] = {w->cin, w->cout, w->d_seg, w->d_chunk, w->d_sc_keys};
-  for (void* p : ptrs) if (p) Q(cudaFree(p));
-  void* pinned[] = {w->h_seg, w->h_chunk, w->h_sc_keys};
-  for (void* p : pinned) if (p) Q(cudaFreeHost(p));
   if (w->ev_seg) Q(cudaEventDestroy(w->ev_seg));
   delete w;
 }
 
-// grow-only device buffer whose contents need not survive: a failure leaves it empty
-static int kf_grow(void** p, size_t* cap, size_t need) {
-  if (need <= *cap) return 0;
-  if (*p) Q(cudaFree(*p));
-  *p = nullptr;
-  *cap = 0;
-  CU(cudaMalloc(p, need + need / 4));
-  *cap = need + need / 4;
-  return 0;
-}
+// growth policy of the key-frame buffers that follow the selection size: a quarter of headroom
+template <typename T>
+static int kf_grow(DevBuf<T>& b, size_t need) { return grow(b, need, need + need / 4); }
 
 // The map's KfWork, created on first use.
 static int kf_work(flb_map* m) {
@@ -65,21 +52,18 @@ static int kf_scratch(flb_map* m, int n, bool curv, bool filter) {
   if (kf_work(m)) return 1;
   KfWork& w = *m->kfw;
   const size_t pts = sizeof(float4) * (size_t)n, cur = sizeof(float) * (size_t)n;
-  if (kf_grow((void**)&m->kf_in, &m->kf_in_cap, pts)) return 1;
-  if (curv && kf_grow((void**)&w.cin, &w.cin_cap, cur)) return 1;
+  if (kf_grow(m->kf_in, pts)) return 1;
+  if (curv && kf_grow(w.cin, cur)) return 1;
   if (!filter) return 0;
-  if (kf_grow((void**)&m->kf_out, &m->kf_out_cap, pts)) return 1;
-  if (curv && kf_grow((void**)&w.cout, &w.cout_cap, cur)) return 1;
+  if (kf_grow(m->kf_out, pts)) return 1;
+  if (curv && kf_grow(w.cout, cur)) return 1;
   return vg_ensure(w.vg, n);
 }
 
 static long long kf_scratch_bytes(const flb_map* m) {
-  size_t b = m->kf_raw_cap + m->kf_in_cap + m->kf_out_cap;
-  if (const KfWork* w = m->kfw) {
-    b += w->cin_cap + w->cout_cap + sizeof(KfSeg) * (size_t)w->seg_cap;
-    b += sizeof(ScChunk) * (size_t)w->chunk_cap + sizeof(unsigned) * SC_BINS * (size_t)w->sc_cap;
-    if (w->vg.cap) b += (2 * sizeof(unsigned) + 4 * sizeof(int)) * (size_t)w->vg.cap + w->vg.tmp_bytes + 8 * sizeof(unsigned);
-  }
+  size_t b = m->kf_raw.cap + m->kf_in.cap + m->kf_out.cap;   // device bytes (the pinned staging is not counted)
+  if (const KfWork* w = m->kfw)
+    b += w->cin.cap + w->cout.cap + w->d_seg.cap + w->d_chunk.cap + w->d_sc_keys.cap + vg_device_bytes(w->vg);
   return (long long)b;
 }
 
@@ -87,10 +71,9 @@ extern "C" int flb_map_release_keyframe_scratch(flb_map* m) {
   if (!m) return set_err("null map");
   CU(cudaSetDevice(m->cfg.device));
   CU(cudaStreamSynchronize(m->stream));
-  void* ptrs[] = {m->kf_raw, m->kf_in, m->kf_out};
-  for (void* p : ptrs) if (p) Q(cudaFree(p));
-  m->kf_raw = nullptr; m->kf_in = m->kf_out = nullptr;
-  m->kf_raw_cap = m->kf_in_cap = m->kf_out_cap = 0;
+  m->kf_raw.release();
+  m->kf_in.release();
+  m->kf_out.release();
   kfw_release(m->kfw);
   m->kfw = nullptr;
   return 0;
@@ -124,17 +107,10 @@ static int kf_upload_segs(flb_map* m, const std::vector<KfSeg>& segs) {
   KfWork& w = *m->kfw;
   const int ns = (int)segs.size();
   CU(cudaEventSynchronize(w.ev_seg));   // the previous table copy has left the pinned staging
-  if (ns > w.seg_cap) {
-    if (w.d_seg) Q(cudaFree(w.d_seg));
-    if (w.h_seg) Q(cudaFreeHost(w.h_seg));
-    w.d_seg = w.h_seg = nullptr; w.seg_cap = 0;
-    const int cap = std::max(ns, 256);
-    CU(cudaMalloc((void**)&w.d_seg, sizeof(KfSeg) * (size_t)cap));
-    CU(cudaMallocHost((void**)&w.h_seg, sizeof(KfSeg) * (size_t)cap));
-    w.seg_cap = cap;
-  }
-  memcpy(w.h_seg, segs.data(), sizeof(KfSeg) * (size_t)ns);
-  CU(cudaMemcpyAsync(w.d_seg, w.h_seg, sizeof(KfSeg) * (size_t)ns, cudaMemcpyHostToDevice, m->stream));
+  const size_t bytes = sizeof(KfSeg) * (size_t)ns, floor = sizeof(KfSeg) * 256;
+  if (grow(w.d_seg, bytes, floor) || grow(w.h_seg, bytes, floor)) return 1;
+  memcpy(w.h_seg.p, segs.data(), bytes);
+  CU(cudaMemcpyAsync(w.d_seg.p, w.h_seg.p, bytes, cudaMemcpyHostToDevice, m->stream));
   CU(cudaEventRecord(w.ev_seg, m->stream));
   return 0;
 }
@@ -144,7 +120,7 @@ static int kf_assemble_enqueue(flb_map* m, const std::vector<KfSeg>& segs, const
                                float* out_curv) {
   if (n == 0) return 0;
   if (kf_upload_segs(m, segs)) return 1;
-  k_kf_assemble<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->kfw->d_seg, (int)segs.size(), src, src_curv, n, out,
+  k_kf_assemble<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->kfw->d_seg.p, (int)segs.size(), src, src_curv, n, out,
                                                                           out_curv);
   m->launches++;
   CU(cudaGetLastError());
@@ -155,11 +131,11 @@ static int kf_assemble_enqueue(flb_map* m, const std::vector<KfSeg>& segs, const
 // (laserMapping.cpp:640-643), ikdtree.reconstruct (:656), featsFromMap->points = subMapKeyFramesDS->points (:664).
 static int kf_rebuild_tail(flb_map* m, int n, float leaf, float* out_xyzi, int cap, int* n_points) {
   VgWork& w = m->kfw->vg;
-  if (vg_enqueue(m, w, m->kf_in, nullptr, n, leaf, m->kf_out, nullptr, n, m->stream)) return 1;
+  if (vg_enqueue(m, w, m->kf_in.p, nullptr, n, leaf, m->kf_out.p, nullptr, n, m->stream)) return 1;
   CU(cudaStreamSynchronize(m->stream));
-  const bool ovf = w.h_mm[6] != 0;
-  const int nd = ovf ? n : (int)w.h_mm[7];
-  const float4* ds = ovf ? m->kf_in : m->kf_out;
+  const bool ovf = w.h_mm.p[6] != 0;
+  const int nd = ovf ? n : (int)w.h_mm.p[7];
+  const float4* ds = ovf ? m->kf_in.p : m->kf_out.p;
   if (n_points) *n_points = nd;
   if (map_reset_storage(m)) return 1;
   if (nd > 0 && insert_device(m, ds, nullptr, nd, 0)) return 1;
@@ -188,7 +164,7 @@ extern "C" int flb_map_reconstruct_keyframes(flb_map* m, const void* const* clou
   const int n = (int)total;
   if (n == 0) return map_reset_storage(m);   // reconstruct with an empty cloud: everything deleted
   if (kf_scratch(m, n, false, true)) return 1;
-  if (kf_grow((void**)&m->kf_raw, &m->kf_raw_cap, (size_t)n * stride)) return 1;
+  if (kf_grow(m->kf_raw, (size_t)n * stride)) return 1;
   // all clouds share the stride: staged back to back, packed by one launch, then transformed by one assembly
   std::vector<KfSeg> segs;
   segs.reserve(n_kf);
@@ -196,15 +172,13 @@ extern "C" int flb_map_reconstruct_keyframes(flb_map* m, const void* const* clou
   for (int k = 0; k < n_kf; ++k) {
     const int c = sizes[k];
     if (c == 0) continue;
-    CU(cudaMemcpyAsync(m->kf_raw + (size_t)off * stride, clouds[k], (size_t)c * stride, cudaMemcpyHostToDevice, m->stream));
+    CU(cudaMemcpyAsync(m->kf_raw.p + (size_t)off * stride, clouds[k], (size_t)c * stride, cudaMemcpyHostToDevice, m->stream));
     segs.push_back(kf_seg(affine_from_rpy(poses6 + 6 * k).t, false, off, (int)off, c));
     off += c;
   }
-  k_pack_xyzic<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->kf_raw, stride, off_intensity, -1, m->kf_out, nullptr, n);
-  m->launches++;
-  CU(cudaGetLastError());
+  if (pack_records(m, m->stream, m->kf_raw.p, n, stride, off_intensity, -1, m->kf_out.p, nullptr)) return 1;
   // *subMapKeyFrames += *transformPointCloud(surfCloudKeyFrames[k], &cloudKeyPoses6D->points[k])  (laserMapping.cpp:636)
-  if (kf_assemble_enqueue(m, segs, m->kf_out, nullptr, n, m->kf_in, nullptr)) return 1;
+  if (kf_assemble_enqueue(m, segs, m->kf_out.p, nullptr, n, m->kf_in.p, nullptr)) return 1;
   return kf_rebuild_tail(m, n, leaf, out_xyzi, cap, n_points);
 }
 
@@ -218,8 +192,7 @@ struct flb_keyframes {
   std::vector<long long> off;        // first point of key frame k
   std::vector<int> cnt;              // its size
   long long n_pts = 0;
-  unsigned char* raw = nullptr;      // staging of host records (flb_keyframes_append)
-  size_t raw_cap = 0;
+  DevBuf<unsigned char> raw;         // staging of host records (flb_keyframes_append)
   bool holds_ref = false;
 };
 
@@ -258,7 +231,7 @@ extern "C" void flb_keyframes_destroy(flb_keyframes* k) {
   flb_map* m = k->map;
   Q(cudaSetDevice(m->cfg.device));
   Q(cudaStreamSynchronize(m->stream));
-  void* ptrs[] = {k->xyzi, k->curv, k->raw};
+  void* ptrs[] = {k->xyzi, k->curv};
   for (void* p : ptrs) if (p) Q(cudaFree(p));
   const bool counted = k->holds_ref;
   delete k;
@@ -305,13 +278,10 @@ extern "C" int flb_keyframes_append(flb_keyframes* k, const void* pts, int n, in
   flb_map* m = k->map;
   CU(cudaSetDevice(m->cfg.device));
   if (n > 0) {
-    const size_t bytes = (size_t)n * stride;
-    if (kf_grow((void**)&k->raw, &k->raw_cap, bytes)) return 1;
-    CU(cudaMemcpyAsync(k->raw, pts, bytes, cudaMemcpyHostToDevice, m->stream));
-    k_pack_xyzic<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(k->raw, stride, off_intensity, off_curvature,
-                                                                          k->xyzi + k->n_pts, k->curv + k->n_pts, n);
-    m->launches++;
-    CU(cudaGetLastError());
+    const size_t bytes = (size_t)n * stride;   // staging with a quarter of headroom, as kf_grow
+    if (upload_records(m, m->stream, k->raw, bytes + bytes / 4, pts, n, stride, off_intensity, off_curvature, k->xyzi + k->n_pts,
+                       k->curv + k->n_pts))
+      return 1;
   }
   kf_commit(k, n, index);
   return 0;
@@ -331,7 +301,7 @@ extern "C" int flb_keyframes_info(const flb_keyframes* k, int* n_keyframes, long
   if (!k) return set_err("null key-frame store");
   if (n_keyframes) *n_keyframes = (int)k->cnt.size();
   if (n_points) *n_points = k->n_pts;
-  if (device_bytes) *device_bytes = (long long)((sizeof(float4) + sizeof(float)) * (size_t)k->cap_pts + k->raw_cap);
+  if (device_bytes) *device_bytes = (long long)((sizeof(float4) + sizeof(float)) * (size_t)k->cap_pts + k->raw.cap);
   if (map_scratch_bytes) *map_scratch_bytes = kf_scratch_bytes(k->map);
   return 0;
 }
@@ -381,7 +351,7 @@ extern "C" int flb_map_reconstruct_from_keyframes(flb_map* m, const flb_keyframe
     segs.push_back(kf_seg(affine_from_rpy(poses6 + 6 * j).t, false, k->off[ids[j]], dst, c));
     dst += c;
   }
-  if (kf_assemble_enqueue(m, segs, k->xyzi, nullptr, n, m->kf_in, nullptr)) return 1;
+  if (kf_assemble_enqueue(m, segs, k->xyzi, nullptr, n, m->kf_in.p, nullptr)) return 1;
   return kf_rebuild_tail(m, n, leaf, out_xyzi, cap, n_points);
 }
 
@@ -429,16 +399,16 @@ extern "C" int flb_keyframes_assemble(flb_keyframes* k, const int* ids, int n_id
   KfWork& w = *m->kfw;
   std::vector<KfSeg> segs;
   kf_selection_segs(k, ids, n_ids, transform_kind, transforms, segs);
-  if (kf_assemble_enqueue(m, segs, k->xyzi, k->curv, n, m->kf_in, w.cin)) return 1;
+  if (kf_assemble_enqueue(m, segs, k->xyzi, k->curv, n, m->kf_in.p, w.cin.p)) return 1;
   if (leaf == 0.f) {   // the dense concatenation (GlobalMap.pcd, the loop sub-maps)
     if (n_out) *n_out = n;
-    return fe_download(m, m->kf_in, w.cin, n, out_xyzi, out_curvature, cap);
+    return fe_download(m, m->kf_in.p, w.cin.p, n, out_xyzi, out_curvature, cap);
   }
   // downSizeFilterSurf / downSizeFilterGlobalMapKeyFrames .filter (laserMapping.cpp:1780-1789, :1866-1869)
-  if (vg_enqueue(m, w.vg, m->kf_in, w.cin, n, leaf, m->kf_out, w.cout, n, m->stream)) return 1;
+  if (vg_enqueue(m, w.vg, m->kf_in.p, w.cin.p, n, leaf, m->kf_out.p, w.cout.p, n, m->stream)) return 1;
   CU(cudaStreamSynchronize(m->stream));
-  const bool ovf = w.vg.h_mm[6] != 0;   // PCL's int32 overflow guard: the input comes back unchanged
-  const int nd = ovf ? n : (int)w.vg.h_mm[7];
+  const bool ovf = w.vg.h_mm.p[6] != 0;   // PCL's int32 overflow guard: the input comes back unchanged
+  const int nd = ovf ? n : (int)w.vg.h_mm.p[7];
   if (n_out) *n_out = nd;
-  return fe_download(m, ovf ? m->kf_in : m->kf_out, ovf ? w.cin : w.cout, nd, out_xyzi, out_curvature, cap);
+  return fe_download(m, ovf ? m->kf_in.p : m->kf_out.p, ovf ? w.cin.p : w.cout.p, nd, out_xyzi, out_curvature, cap);
 }

@@ -600,14 +600,6 @@ __global__ void k_rehash_insert(MapDev m, int nblk) {
   }
 }
 
-// strided host points -> float4 (x, y, z, intensity); off_i < 0: no intensity in the records (0)
-__global__ void k_pack_points(const unsigned char* __restrict__ src, int stride, int off_i, float4* dst, int n) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const float* p = reinterpret_cast<const float*>(src + (size_t)i * stride);
-    const float w = off_i >= 0 ? *reinterpret_cast<const float*>(src + (size_t)i * stride + off_i) : 0.f;
-    dst[i] = make_float4(p[0], p[1], p[2], w);
-  }
-}
 // intensity of returned neighbours (API searches only; off the hot path): the neighbour's voxel is re-read and the point with
 // exactly these coordinates looked up.  pts: (x, y, z, d2) records, NaN x = no neighbour.
 __global__ void k_lookup_intensity(MapDev m, const float4* __restrict__ pts, float* __restrict__ out, int n) {

@@ -5,47 +5,26 @@
 
 // scratch of the preprocess call that the front end does not already own (allocated on first use, grown only)
 struct PpWork {
-  int cap = 0;          // points
-  int ring_cap = 0;     // rings
-  double* yaw = nullptr;
-  int* ring_first = nullptr;
-  void* tmp = nullptr;
-  size_t tmp_bytes = 0;
-  PpOut* d_out = nullptr;
-  PpOut* h_out = nullptr;   // pinned
+  int cap = 0;                 // points yaw and the CUB scratch are sized for
+  DevBuf<double> yaw;
+  DevBuf<int> ring_first;
+  DevBuf<unsigned char> tmp;   // CUB temporary storage
+  DevBuf<PpOut> d_out;
+  PinnedBuf<PpOut> h_out;
 };
-static void pp_release(PpWork* w) {
-  if (!w) return;
-  void* ptrs[] = {w->yaw, w->ring_first, w->tmp, w->d_out};
-  for (void* p : ptrs) if (p) Q(cudaFree(p));
-  if (w->h_out) Q(cudaFreeHost(w->h_out));
-  delete w;
-}
+static void pp_release(PpWork* w) { delete w; }
 static int pp_ensure(PpWork& w, int cap, int rings) {
-  if (!w.d_out) {
-    CU(cudaMalloc((void**)&w.d_out, sizeof(PpOut)));
-    CU(cudaMallocHost((void**)&w.h_out, sizeof(PpOut)));
-  }
+  if (grow(w.d_out, sizeof(PpOut), 0) || grow(w.h_out, sizeof(PpOut), 0)) return 1;
   if (cap > w.cap) {
-    if (w.yaw) Q(cudaFree(w.yaw));
-    if (w.tmp) Q(cudaFree(w.tmp));
-    w.yaw = nullptr; w.tmp = nullptr; w.cap = 0;
+    w.cap = 0;   // (until both have grown)
     size_t t1 = 0, t2 = 0;
     CU(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr,
                                        cap, 0, 16));
     CU(cub::DeviceScan::InclusiveScan(nullptr, t2, (const unsigned*)nullptr, (unsigned*)nullptr, PpMapCompose(), cap));
-    w.tmp_bytes = std::max(t1, t2) + 256;
-    CU(cudaMalloc((void**)&w.yaw, sizeof(double) * (size_t)cap));
-    CU(cudaMalloc(&w.tmp, w.tmp_bytes));
+    if (grow(w.yaw, sizeof(double) * (size_t)cap, 0) || grow(w.tmp, std::max(t1, t2) + 256, 0)) return 1;
     w.cap = cap;
   }
-  if (rings > w.ring_cap) {
-    if (w.ring_first) Q(cudaFree(w.ring_first));
-    w.ring_first = nullptr; w.ring_cap = 0;
-    CU(cudaMalloc((void**)&w.ring_first, sizeof(int) * (size_t)rings));
-    w.ring_cap = rings;
-  }
-  return 0;
+  return grow(w.ring_first, sizeof(int) * (size_t)rings, 0);
 }
 
 static int pp_check_field(const char* name, int off, int size, int stride, bool required) {
@@ -113,47 +92,49 @@ extern "C" int flb_frontend_preprocess(flb_frontend* f, const flb_preprocess_con
   }
   PpWork& w = *f->pp;
   if (pp_ensure(w, f->cap, rings)) return 1;
-  if (fe_stage_raw(f, m, records, n, s)) return 1;   // the one H2D copy
+  // the one H2D copy, into the front end's staging (sized once for its capacity)
+  if (grow(f->raw, (size_t)n * s, (size_t)f->cap * s)) return 1;
+  CU(cudaMemcpyAsync(f->raw.p, records, (size_t)n * s, cudaMemcpyHostToDevice, m->stream));
 
   cudaStream_t st = m->stream;
   const int g = grid_for(n, 256, m->sm_count * 8);
   VgWork& v = f->vg;   // its arrays hold max_raw_points entries; free between front-end calls
-  int* keep = v.flags;
-  int* pos = v.pos;
-  CU(cudaMemsetAsync(w.d_out, 0, sizeof(PpOut), st));
+  int* keep = v.flags.p;
+  int* pos = v.pos.p;
+  CU(cudaMemsetAsync(w.d_out.p, 0, sizeof(PpOut), st));
   if (type == PP_OUST64) {
-    k_pp_ouster<<<g, 256, 0, st>>>(f->raw, p, f->pts_t, f->curv_t, keep);
+    k_pp_ouster<<<g, 256, 0, st>>>(f->raw.p, p, f->pts_t, f->curv_t, keep);
     m->launches++;
   } else if (type == PP_VELO16) {
-    if (synth) CU(cudaMemsetAsync(w.ring_first, 0x7F, sizeof(int) * (size_t)rings, st));   // 0x7F7F7F7F > any index
-    k_pp_velo<<<g, 256, 0, st>>>(f->raw, p, synth ? 1 : 0, f->pts_t, f->curv_t, keep, v.keys_a, v.vals_a, w.yaw, w.ring_first, w.d_out);
+    if (synth) CU(cudaMemsetAsync(w.ring_first.p, 0x7F, sizeof(int) * (size_t)rings, st));   // 0x7F7F7F7F > any index
+    k_pp_velo<<<g, 256, 0, st>>>(f->raw.p, p, synth ? 1 : 0, f->pts_t, f->curv_t, keep, v.keys_a.p, v.vals_a.p, w.yaw.p, w.ring_first.p, w.d_out.p);
     m->launches++;
     if (synth) {
       int end_bit = 1;
       while (end_bit < 17 && (1 << end_bit) <= rings) ++end_bit;   // keys are min(ring, n_scans) <= rings
-      size_t tb = w.tmp_bytes;
-      CU(cub::DeviceRadixSort::SortPairs(w.tmp, tb, (const unsigned*)v.keys_a, v.keys_b, (const int*)v.vals_a, v.vals_b, n, 0, end_bit, st));
-      k_pp_velo_maps<<<g, 256, 0, st>>>(v.keys_b, v.vals_b, w.yaw, w.ring_first, p, v.keys_a);
-      tb = w.tmp_bytes;
-      CU(cub::DeviceScan::InclusiveScan(w.tmp, tb, (const unsigned*)v.keys_a, (unsigned*)v.vals_a, PpMapCompose(), n, st));
-      k_pp_velo_apply<<<g, 256, 0, st>>>(v.keys_b, v.vals_b, w.yaw, w.ring_first, (const unsigned*)v.vals_a, p, f->curv_t, keep);
+      size_t tb = w.tmp.cap;
+      CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)v.keys_a.p, v.keys_b.p, (const int*)v.vals_a.p, v.vals_b.p, n, 0, end_bit, st));
+      k_pp_velo_maps<<<g, 256, 0, st>>>(v.keys_b.p, v.vals_b.p, w.yaw.p, w.ring_first.p, p, v.keys_a.p);
+      tb = w.tmp.cap;
+      CU(cub::DeviceScan::InclusiveScan(w.tmp.p, tb, (const unsigned*)v.keys_a.p, (unsigned*)v.vals_a.p, PpMapCompose(), n, st));
+      k_pp_velo_apply<<<g, 256, 0, st>>>(v.keys_b.p, v.vals_b.p, w.yaw.p, w.ring_first.p, (const unsigned*)v.vals_a.p, p, f->curv_t, keep);
       m->launches += 3 + 4 + 2;   // + CUB's radix sort and scan kernels
     }
   } else {
-    k_pp_livox<<<g, 256, 0, st>>>(f->raw, p, f->pts_t, f->curv_t, v.vals_a);
-    size_t tb = v.tmp_bytes;
-    CU(cub::DeviceScan::ExclusiveSum(v.tmp, tb, (const int*)v.vals_a, v.vals_b, n, st));
-    k_pp_livox_keep<<<g, 256, 0, st>>>(f->pts_t, v.vals_a, v.vals_b, p, keep);
+    k_pp_livox<<<g, 256, 0, st>>>(f->raw.p, p, f->pts_t, f->curv_t, v.vals_a.p);
+    size_t tb = v.tmp.cap;
+    CU(cub::DeviceScan::ExclusiveSum(v.tmp.p, tb, (const int*)v.vals_a.p, v.vals_b.p, n, st));
+    k_pp_livox_keep<<<g, 256, 0, st>>>(f->pts_t, v.vals_a.p, v.vals_b.p, p, keep);
     m->launches += 2 + 2;
   }
-  size_t tb = v.tmp_bytes;
-  CU(cub::DeviceScan::ExclusiveSum(v.tmp, tb, (const int*)keep, pos, n, st));
-  k_pp_scatter<<<g, 256, 0, st>>>(f->pts_t, f->curv_t, keep, pos, n, f->pts, f->curv, w.d_out);
+  size_t tb = v.tmp.cap;
+  CU(cub::DeviceScan::ExclusiveSum(v.tmp.p, tb, (const int*)keep, pos, n, st));
+  k_pp_scatter<<<g, 256, 0, st>>>(f->pts_t, f->curv_t, keep, pos, n, f->pts, f->curv, w.d_out.p);
   m->launches += 1 + 2;
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(w.h_out, w.d_out, sizeof(PpOut), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(w.h_out.p, w.d_out.p, sizeof(PpOut), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
-  const PpOut r = *w.h_out;
+  const PpOut r = *w.h_out.p;
   if (r.bad_ring)
     return set_err("flb_frontend_preprocess: ring %d >= n_scans=%d (scan_line does not match the sensor)", r.bad_ring - 1, cfg->n_scans);
   f->n_raw = r.count;

@@ -12,25 +12,10 @@
 static int sc_scratch(flb_map* m, int n_chunks, int n_desc) {
   if (kf_work(m)) return 1;
   KfWork& w = *m->kfw;
-  if (n_chunks > w.chunk_cap) {
-    if (w.d_chunk) Q(cudaFree(w.d_chunk));
-    if (w.h_chunk) Q(cudaFreeHost(w.h_chunk));
-    w.d_chunk = w.h_chunk = nullptr; w.chunk_cap = 0;
-    const int cap = std::max(n_chunks, 1024);
-    CU(cudaMalloc((void**)&w.d_chunk, sizeof(ScChunk) * (size_t)cap));
-    CU(cudaMallocHost((void**)&w.h_chunk, sizeof(ScChunk) * (size_t)cap));
-    w.chunk_cap = cap;
-  }
-  if (n_desc > w.sc_cap) {
-    if (w.d_sc_keys) Q(cudaFree(w.d_sc_keys));
-    if (w.h_sc_keys) Q(cudaFreeHost(w.h_sc_keys));
-    w.d_sc_keys = w.h_sc_keys = nullptr; w.sc_cap = 0;
-    const size_t bytes = sizeof(unsigned) * SC_BINS * (size_t)n_desc;
-    CU(cudaMalloc((void**)&w.d_sc_keys, bytes));
-    CU(cudaMallocHost((void**)&w.h_sc_keys, bytes));
-    w.sc_cap = n_desc;
-  }
-  return 0;
+  const size_t chunks = sizeof(ScChunk) * (size_t)n_chunks, chunk_floor = sizeof(ScChunk) * 1024;
+  const size_t keys = sizeof(unsigned) * SC_BINS * (size_t)n_desc;
+  if (grow(w.d_chunk, chunks, chunk_floor) || grow(w.h_chunk, chunks, chunk_floor)) return 1;
+  return grow(w.d_sc_keys, keys, 0) || grow(w.h_sc_keys, keys, 0);
 }
 
 // The float a key stands for, as a double; key 0 (no point beat -1000) is the reference's NO_POINT reset to 0.
@@ -56,18 +41,18 @@ static int sc_run(flb_keyframes* k, const std::vector<KfSeg>& segs, const std::v
   if (sc_scratch(m, nc, n_desc)) return 1;
   KfWork& w = *m->kfw;
   const size_t key_bytes = sizeof(unsigned) * SC_BINS * (size_t)n_desc;
-  CU(cudaMemsetAsync(w.d_sc_keys, 0, key_bytes, m->stream));
+  CU(cudaMemsetAsync(w.d_sc_keys.p, 0, key_bytes, m->stream));
   if (nc > 0) {
     if (kf_upload_segs(m, segs)) return 1;
-    memcpy(w.h_chunk, chunks.data(), sizeof(ScChunk) * (size_t)nc);   // free: every call ends in a synchronisation
-    CU(cudaMemcpyAsync(w.d_chunk, w.h_chunk, sizeof(ScChunk) * (size_t)nc, cudaMemcpyHostToDevice, m->stream));
-    k_sc_bins<<<std::min(nc, m->sm_count * 8), 256, 0, m->stream>>>(w.d_seg, w.d_chunk, nc, k->xyzi, lidar_height, w.d_sc_keys);
+    memcpy(w.h_chunk.p, chunks.data(), sizeof(ScChunk) * (size_t)nc);   // free: every call ends in a synchronisation
+    CU(cudaMemcpyAsync(w.d_chunk.p, w.h_chunk.p, sizeof(ScChunk) * (size_t)nc, cudaMemcpyHostToDevice, m->stream));
+    k_sc_bins<<<std::min(nc, m->sm_count * 8), 256, 0, m->stream>>>(w.d_seg.p, w.d_chunk.p, nc, k->xyzi, lidar_height, w.d_sc_keys.p);
     m->launches++;
     CU(cudaGetLastError());
   }
-  CU(cudaMemcpyAsync(w.h_sc_keys, w.d_sc_keys, key_bytes, cudaMemcpyDeviceToHost, m->stream));
+  CU(cudaMemcpyAsync(w.h_sc_keys.p, w.d_sc_keys.p, key_bytes, cudaMemcpyDeviceToHost, m->stream));
   CU(cudaStreamSynchronize(m->stream));
-  for (size_t b = 0; b < (size_t)SC_BINS * n_desc; ++b) out[b] = sc_value(w.h_sc_keys[b]);
+  for (size_t b = 0; b < (size_t)SC_BINS * n_desc; ++b) out[b] = sc_value(w.h_sc_keys.p[b]);
   return 0;
 }
 
