@@ -247,7 +247,8 @@ __global__ void k_esikf_begin(EsikfCtl* c, const double* __restrict__ stage, int
     sst[2 * i] = v.x;
     sst[2 * i + 1] = v.y;
   }
-  if (threadIdx.x >= 32 && threadIdx.x < 48) work_counts[threadIdx.x - 32] = 0;   // per-pass k-NN work-list counters [0..7] + tickets [8..15]
+  // per-pass k-NN work-list counters [0..7], tickets [8..15] and stencil CTAs done [16..23]
+  if (threadIdx.x >= 32 && threadIdx.x < 56) work_counts[threadIdx.x - 32] = 0;
   __syncthreads();
   const double* x0 = sst;
   const double* P0 = sst + 26;

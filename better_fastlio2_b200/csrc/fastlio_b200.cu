@@ -89,23 +89,30 @@ extern "C" int flb_device_count(void) {
   return n;
 }
 
-// Kernel launch of the scan sequence.  FLB_PDL=1 adds the programmatic-stream-serialization attribute (programmatic
-// dependent launch: a kernel's launch overlaps its predecessor's tail; the kernels call pdl_sync() before touching
-// anything; under stream capture the attribute becomes a programmatic graph edge).  OFF by default, kept as an A/B switch.
-static bool pdl_enabled() {
-  static const bool on = [] { const char* e = getenv("FLB_PDL"); return e && atoi(e) != 0; }();
-  return on;
-}
+// Kernel launch with or without the programmatic-stream-serialization attribute (programmatic dependent launch: the
+// kernel's CTAs may start once every CTA of its predecessor has run griddepcontrol.launch_dependents; under stream capture
+// the attribute becomes a programmatic graph edge).
 template <typename... P, typename... A>
-static cudaError_t launch_k(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+static cudaError_t launch_kx(bool programmatic, void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = programmatic ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<P>(args)...);
+}
+// Kernel launch of the scan sequence.  FLB_PDL=1 launches it programmatically (a kernel's launch overlaps its
+// predecessor's tail; the kernels call pdl_sync() before touching anything).  OFF by default, kept as an A/B switch; the
+// exact k-NN kernel is always launched programmatically after the stencil kernel (launch_knn).
+static bool pdl_enabled() {
+  static const bool on = [] { const char* e = getenv("FLB_PDL"); return e && atoi(e) != 0; }();
+  return on;
+}
+template <typename... P, typename... A>
+static cudaError_t launch_k(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+  return launch_kx(pdl_enabled(), kern, grid, block, smem, st, static_cast<A&&>(args)...);
 }
 
 static inline uint32_t next_pow2(uint64_t v) {
@@ -231,9 +238,10 @@ static int fetch_counters(flb_map* m) {
   CU(cudaStreamSynchronize(m->stream));
   const int e = absorb_range_flag(m);
   if (e) {
-    return set_err("device map error flags 0x%x:%s%s%s%s%s", e, (e & ERR_BLOCKS_FULL) ? " block pool exhausted (raise max_blocks)" : "",
+    return set_err("device map error flags 0x%x:%s%s%s%s%s%s", e, (e & ERR_BLOCKS_FULL) ? " block pool exhausted (raise max_blocks)" : "",
                    (e & ERR_OVF_FULL) ? " overflow pool exhausted (raise max_points)" : "", (e & ERR_HASH_FULL) ? " block hash full" : "",
-                   (e & ERR_COARSE_FULL) ? " coarse hash full" : "", (e & ERR_RANGE) ? " point outside representable range / NaN" : "");
+                   (e & ERR_COARSE_FULL) ? " coarse hash full" : "", (e & ERR_RANGE) ? " point outside representable range / NaN" : "",
+                   (e & ERR_KNN_STALL) ? " k-NN work-list wait timed out" : "");
   }
   return 0;
 }
@@ -281,7 +289,9 @@ extern "C" int flb_map_create(const flb_map_config* cfg, flb_map** out) {
   rc |= dev_alloc(m, (void**)&d.cbits, sizeof(uint64_t) * 8 * (size_t)m->chash_cap);
   rc |= dev_alloc(m, (void**)&d.clist, sizeof(uint32_t) * (size_t)m->chash_cap);
   rc |= dev_alloc(m, (void**)&d.counters, sizeof(int) * CNT_COUNT);
-  rc |= dev_alloc(m, (void**)&m->d_misc, sizeof(int) * 32);   // [0..3] counts, [4..9] range, [12] work count, [13] ticket, [16..23] per-pass work counts, [24..31] per-pass tickets
+  // d_misc: [0..3] counts, [4..9] range, [12] work count, [13] ticket, [14] stencil CTAs done, [16..23] per-pass work counts,
+  // [24..31] per-pass tickets, [32..39] per-pass stencil CTAs done
+  rc |= dev_alloc(m, (void**)&m->d_misc, sizeof(int) * 48);
   rc |= dev_alloc(m, (void**)&m->d_phase, sizeof(int) * 8);
   if (rc) { flb_map_destroy(m); return 1; }
   if (cudaMallocHost((void**)&m->h_counters, sizeof(int) * CNT_COUNT) != cudaSuccess) { flb_map_destroy(m); return set_err("cudaMallocHost failed"); }
@@ -382,11 +392,16 @@ static int ensure_scratch(flb_map* m, int n) {
   return 0;
 }
 
-// the stencil k-NN kernel's work list for n queries; a captured scan graph holds its address
+// warps of the exact k-NN kernel's grid (launch_knn)
+static int exact_warps(const flb_map* m, int K) { return m->exact_ctas[K == 5 ? 0 : 1] * (KNN_THREADS / 32); }
+
+// the stencil k-NN kernel's work list for n queries and the entries that close it (one per exact-kernel warp), all
+// WORK_EMPTY (0xFF bytes); a captured scan graph holds its address
 static int ensure_worklist(flb_map* m, int n) {
-  const size_t need = sizeof(int) * (size_t)n;
+  const size_t need = sizeof(int) * ((size_t)n + std::max(exact_warps(m, 5), exact_warps(m, 20)));
   if (need <= m->worklist.cap) return 0;
   if (grow(m->worklist, need, sizeof(int) << 17)) return 1;
+  CU(cudaMemsetAsync(m->worklist.p, 0xFF, m->worklist.cap, m->stream));
   m->gen++;
   return 0;
 }
@@ -559,15 +574,19 @@ static int launch_knn(flb_map* m, KnnArgs a) {
   if (!a.work_count) {   // (device-driven scans use per-pass counters zeroed by k_esikf_begin: no memset node per pass)
     a.work_count = m->d_misc + 12;
     a.work_ticket = m->d_misc + 13;
-    CU(cudaMemsetAsync(a.work_count, 0, 2 * sizeof(int), m->stream));
+    a.stencil_done = m->d_misc + 14;
+    CU(cudaMemsetAsync(a.work_count, 0, 3 * sizeof(int), m->stream));
   }
+  a.exact_warps = exact_warps(m, K);
   // one thread per query (a.n is the session capacity on the device-driven path; CTAs past the scan's size exit at once).
   // A cfg2 scan (~930 CTAs) is a little more than the 924 CTAs an H100 holds at 7 per SM.  Two ways to make it one wave
   // were measured slower (DESIGN.md §3): a resident grid looping over warp-sized chunks claimed by ticket (the loop cost
   // ~250 B of register spills per thread) and a 64-register cap for 8 CTAs per SM (~100 B of spills).
   launch_k(k_knn_stencil<K>, (a.n + 127) / 128, 128, 0, m->stream, a);
-  // the exact completion: all CTAs resident (from the occupancy API), looping over the work list
-  launch_k(k_knn<K>, m->exact_ctas[K == 5 ? 0 : 1], KNN_THREADS, 0, m->stream, a);
+  // the exact completion: all CTAs resident (from the occupancy API), looping over the work list.  A programmatic
+  // dependent of the stencil kernel: its CTAs start on the SMs the stencil kernel's early CTAs leave, and take the
+  // unresolved queries as they are published (work-list hand-over, knn_kernels.cuh)
+  launch_kx(true, k_knn<K>, m->exact_ctas[K == 5 ? 0 : 1], KNN_THREADS, 0, m->stream, a);
   m->launches += 2;
   return 0;
 }
@@ -784,7 +803,8 @@ extern "C" int flb_debug_knn_bench(flb_map* m, const float* q_xyz, int nq, int s
   CU(cudaMalloc((void**)&dcnt, nq));
   KnnArgs a;
   a.m = m->d; a.q = m->stage.p; a.n = nq; a.nbr = m->outbuf.p; a.cnt = dcnt; a.max_d2 = INFINITY; a.phase_stats = nullptr;
-  a.worklist = m->worklist.p; a.work_count = m->d_misc + 12; a.work_ticket = m->d_misc + 13; a.ctl = nullptr; a.body = nullptr; a.stride = nq;
+  a.worklist = m->worklist.p; a.work_count = m->d_misc + 12; a.work_ticket = m->d_misc + 13; a.stencil_done = m->d_misc + 14;
+  a.exact_warps = exact_warps(m, 5); a.ctl = nullptr; a.body = nullptr; a.stride = nq;
   cudaError_t e = cudaFuncSetAttribute(k_knn_tile<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (e == cudaSuccess) e = cudaEventCreate(&e0);
@@ -792,13 +812,15 @@ extern "C" int flb_debug_knn_bench(flb_map* m, const float* q_xyz, int nq, int s
   const int grid = (nq + 127) / 128;
   for (int it = -2; it < iters && e == cudaSuccess; ++it) {
     if (it == 0) e = cudaEventRecord(e0, m->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a.work_count, 0, 2 * sizeof(int), m->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.work_count, 0, 3 * sizeof(int), m->stream);
     if (variant == 0) k_knn_stencil<5><<<grid, 128, 0, m->stream>>>(a);
     else k_knn_tile<5><<<grid, TILE_THREADS, sizeof(TileSmem), m->stream>>>(a);
     if (e == cudaSuccess) e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaEventRecord(e1, m->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
+  // nothing consumed the list: leave it empty for the next search
+  if (e == cudaSuccess) e = cudaMemsetAsync(m->worklist.p, 0xFF, m->worklist.cap, m->stream);
   float ms = 0.f;
   if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, e0, e1);
   if (ms_per_launch) *ms_per_launch = ms / (float)iters;
@@ -1304,6 +1326,7 @@ static int enqueue_scan_device(flb_session* s, bool with_insert) {
       a.m = m->d; a.q = nullptr; a.n = cap; a.nbr = s->nbr; a.cnt = s->cnt; a.max_d2 = INFINITY;
       a.phase_stats = m->prof_on ? m->d_phase : nullptr;
       a.ctl = s->ctl; a.body = nullptr; a.stride = cap; a.work_count = p < 8 ? m->d_misc + 16 + p : nullptr; a.work_ticket = p < 8 ? m->d_misc + 24 + p : nullptr;
+      a.stencil_done = p < 8 ? m->d_misc + 32 + p : nullptr;
       if (launch_knn<5>(m, a)) return 1;
     }
     {

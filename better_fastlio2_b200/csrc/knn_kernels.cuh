@@ -183,8 +183,11 @@ struct KnnArgs {
   float max_d2;        // max_dist^2 (INF: unbounded)
   int* phase_stats;    // optional [4]: queries finishing in phase A / B / C, total candidate points
   int* worklist;       // stencil kernel: indices of queries it could not prove complete; warp kernel: its input list
+                       // (WORK_EMPTY between passes; see "work-list hand-over" below)
   int* work_count;     // number of entries in worklist (device)
   int* work_ticket;    // exact kernel: next unclaimed work-list entry (device, zeroed with work_count)
+  int* stencil_done;   // stencil CTAs holding queries that have published all of them (device, zeroed with work_count)
+  int exact_warps;     // warps of the exact kernel's grid: the stencil kernel closes that many entries past the list's end
   const EsikfCtl* ctl; // device-driven mode: queries = body_to_world(ctl->pose, ctl->body[i]); skipped unless a search pass
   const float4* body;  // (unused: the scan pointer of the device-driven mode is ctl->body)
   int stride;          // leading dimension of nbr (>= n; the session capacity, so launches do not depend on n)
@@ -488,6 +491,48 @@ __device__ __noinline__ void warp_finish_coarse(MapDev m, unsigned* cand, unsign
     }
 }
 
+// Work-list hand-over.  The exact kernel is launched as a programmatic dependent of the stencil kernel: its CTAs become
+// resident while the stencil kernel's slowest warps are still running, and take unresolved queries as they are published.
+//   stencil thread: writes the query's neighbour cache and count, takes an entry with atomicAdd(work_count) and stores the
+//     query index into it with a release store.  Each CTA holding queries then counts itself into stencil_done; the CTA
+//     that completes the count (every entry is published by then) closes the list: it writes WORK_END into the
+//     exact_warps entries past its end.
+//   exact warp: holds one ticket (entry index) at a time, waits until its entry is no longer WORK_EMPTY (relaxed polls,
+//     then one acquire), resets it to WORK_EMPTY and works on it or, at WORK_END, exits.  Tickets are handed out in order and a warp claims
+//     a new one only after finishing one, so when the list is closed the warps hold exactly the closed entries: every
+//     entry is consumed and the list is left all WORK_EMPTY for the next pass.
+//   Launched the ordinary way (no programmatic edge), the exact kernel finds the whole list published and closed.
+constexpr int WORK_EMPTY = -1;
+constexpr int WORK_END = -2;
+constexpr unsigned long long KNN_WAIT_NS = 1000000000ull;   // a wait longer than 1 s is a protocol failure: ERR_KNN_STALL
+
+// Ticket w of the exact kernel (warp-uniform): the query index of entry w, or -1 at the end of the list.
+__device__ __forceinline__ int worklist_take(const KnnArgs& a, int w, int lane) {
+  int v = WORK_EMPTY;
+  if (lane == 0) {
+    v = ld_relaxed(&a.worklist[w]);
+    if (v == WORK_EMPTY) {
+      // not published yet: back off with sleeps, so that waiting warps leave the issue slots to the stencil kernel's warps
+      const unsigned long long t0 = global_timer_ns();
+      unsigned ns = 32;
+      do {
+        __nanosleep(ns);
+        ns = min(2u * ns, 512u);
+        v = ld_relaxed(&a.worklist[w]);
+        if (v == WORK_EMPTY && global_timer_ns() - t0 > KNN_WAIT_NS) {
+          atomicOr(&a.m.counters[CNT_ERROR], ERR_KNN_STALL);
+          v = WORK_END;
+        }
+      } while (v == WORK_EMPTY);
+    }
+    if (v >= 0) v = ld_acquire(&a.worklist[w]);   // the one acquire of this entry (same value: only this warp resets it)
+    a.worklist[w] = WORK_EMPTY;   // (this warp is the entry's only reader; its next writer is a later kernel)
+  }
+  v = __shfl_sync(FULL, v, 0);
+  __syncwarp();   // the acquire of lane 0 orders the other lanes' reads of the query's neighbour cache
+  return v == WORK_END ? -1 : v;
+}
+
 // K1b: exact completion of the queries the stencil kernel could not prove complete (its work list).  The stencil
 // kernel has already visited the whole 5x5x5 voxel stencil and left its (up to K) best points in the neighbour cache:
 // they seed the search, which then only looks OUTSIDE the stencil.  One WARP per query, work claimed by atomic tickets.
@@ -508,9 +553,12 @@ __device__ __noinline__ void warp_finish_coarse(MapDev m, unsigned* cand, unsign
 //   Queries still open after ring EXACT_RINGS (nothing within ~6 m at 0.2 m voxels: far outside the map) are finished over
 //   the coarse levels by warp_finish_coarse (remaining blocks of the 3x3x3 coarse cells, then every coarse cell with
 //   box-distance pruning).
+// Launched as a programmatic dependent of k_knn_stencil (work-list hand-over above): no griddepcontrol.wait before the
+// loop (everything but the work list and the neighbour cache was written before the stencil kernel started), and one
+// at the end, so that this grid completes only after the stencil grid and the next kernel sees both grids' writes.
 template <int K>
 __global__ void __launch_bounds__(KNN_THREADS, KNN_MIN_CTAS) k_knn(KnnArgs a) {
-  pdl_sync();
+  pdl_trigger();
   __shared__ ExactSmem sm;
   const MapDev& m = a.m;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -518,27 +566,37 @@ __global__ void __launch_bounds__(KNN_THREADS, KNN_MIN_CTAS) k_knn(KnnArgs a) {
   const float lim = a.max_d2;
   unsigned* cand = sm.cand[wid];
   unsigned long long* cb = sm.cbits[wid];
-  FLB_TRACE_BEGIN(3 * 8 + (a.ctl ? a.ctl->it + 1 : 0));
-  if (a.ctl && !(ctl_pass_active(a.ctl) && a.ctl->converge)) return;
-  const int nwork = *a.work_count;
+  // (the pass's stencil kernel skips the same passes, and a scan without points publishes nothing)
+  const bool active = !(a.ctl && !(ctl_pass_active(a.ctl) && a.ctl->converge)) && (a.ctl ? a.ctl->n : a.n) > 0;
+#ifdef FLB_TRACE
+  const int tslot = 3 * 8 + (a.ctl ? a.ctl->it + 1 : 0);   // timeline of this kernel: first pick-up -> last warp's exit
+  bool first_take = true;
+#endif
   // Dynamic distribution: every warp claims the next list entry with one atomic.  Query cost varies by two orders of
   // magnitude (ring 1 vs far outside the map), so a static stride leaves the kernel waiting for the unlucky warp.
   // (the first entry of every warp is static — its global warp index — so that a few thousand warps do not start by queueing
   // on one atomic; only the entries beyond the first wave are claimed by ticket)
   const int nwarps = (int)(gridDim.x * (blockDim.x >> 5));
   int w = (int)(blockIdx.x * (blockDim.x >> 5)) + wid;
-  for (;; ) {
-    if (w >= nwork) break;   // warp-uniform
-    const int i = a.worklist[w];
+  for (; active; ) {
+    const int i = worklist_take(a, w, lane);   // warp-uniform
+    if (i < 0) break;
+#ifdef FLB_TRACE
+    if (lane == 0) {
+      if (first_take) FLB_TRACE_STAMP(tslot, true);
+      if (a.ctl && a.ctl->it == -1) FLB_TRACE_HIST(80, 2 * 8);   // when the first pass's unresolved queries are picked up
+    }
+    first_take = false;
+#endif
     const float4 q4 = a.ctl ? body_to_world(a.ctl->pose, __ldg(&a.ctl->body[i])) : __ldg(&a.q[i]);
     const float qx = q4.x, qy = q4.y, qz = q4.z;
     TopK<K> t;
     t.clear();
     float rd = CUDART_INF_F, rx = CUDART_NAN_F, ry = CUDART_NAN_F, rz = CUDART_NAN_F, thr = CUDART_INF_F;
     // ---------------- seed: the stencil kernel's result (state as after a merge: lane r holds result r)
-    int gcount = a.cnt[i];
+    int gcount = __ldcg(&a.cnt[i]);   // (L2 loads: written by the stencil kernel while this one runs)
     if (lane < gcount) {
-      const float4 sd = a.nbr[(size_t)lane * a.stride + i];   // plain load: written by the preceding kernel
+      const float4 sd = __ldcg(&a.nbr[(size_t)lane * a.stride + i]);
       rd = sd.w; rx = sd.x; ry = sd.y; rz = sd.z;
       t.d[0] = rd; t.x[0] = rx; t.y[0] = ry; t.z[0] = rz;
     }
@@ -627,7 +685,10 @@ __global__ void __launch_bounds__(KNN_THREADS, KNN_MIN_CTAS) k_knn(KnnArgs a) {
     if (lane == 0) w = nwarps + atomicAdd(a.work_ticket, 1);
     w = __shfl_sync(FULL, w, 0);
   }
-  FLB_TRACE_END(3 * 8 + (a.ctl ? a.ctl->it + 1 : 0));
+  pdl_wait();
+#ifdef FLB_TRACE
+  if (lane == 0 && active) FLB_TRACE_STAMP(tslot, false);
+#endif
 }
 
 // K1a: phase A with ONE THREAD per query (the common case: >99 % of LiDAR returns lie on mapped surfaces and are
@@ -822,16 +883,10 @@ __device__ __forceinline__ void stencil_shell_pass(const MapDev& m, StencilSmem&
   }
 }
 
+// One query of the stencil kernel: search, write the neighbour cache, publish the query if it is unresolved.
 template <int K>
-__global__ void __launch_bounds__(STENCIL_THREADS, 7) k_knn_stencil(KnnArgs a) {
-  pdl_sync();
-  __shared__ StencilSmem sm;
+__device__ __forceinline__ void stencil_query(const KnnArgs& a, StencilSmem& sm, int tid, int i) {
   const MapDev& m = a.m;
-  const int tid = threadIdx.x;
-  const int i = blockIdx.x * blockDim.x + tid;
-  FLB_TRACE_BEGIN(2 * 8 + (a.ctl ? a.ctl->it + 1 : 0));
-  if (a.ctl && !(ctl_pass_active(a.ctl) && a.ctl->converge)) return;
-  if (i >= (a.ctl ? a.ctl->n : a.n)) return;
   const float ds = m.ds;
   const float lim = a.max_d2;
   const float4 q4 = a.ctl ? body_to_world(a.ctl->pose, __ldg(&a.ctl->body[i])) : __ldg(&a.q[i]);
@@ -944,7 +999,37 @@ __global__ void __launch_bounds__(STENCIL_THREADS, 7) k_knn_stencil(KnnArgs a) {
   if (done) {
     if (a.phase_stats) atomicAdd(&a.phase_stats[0], 1);
   } else {
-    a.worklist[atomicAdd(a.work_count, 1)] = i;
+    // the exact kernel may already be waiting for this entry: the release orders the neighbour cache and count before it
+    st_release(&a.worklist[atomicAdd(a.work_count, 1)], i);
+#ifdef FLB_TRACE
+    if (a.ctl && a.ctl->it == -1) FLB_TRACE_HIST(64, 2 * 8);   // when the first pass's unresolved queries are published
+#endif
+  }
+}
+
+template <int K>
+__global__ void __launch_bounds__(STENCIL_THREADS, 7) k_knn_stencil(KnnArgs a) {
+  pdl_sync();
+  __shared__ StencilSmem sm;
+  const int tid = threadIdx.x;
+  FLB_TRACE_BEGIN(2 * 8 + (a.ctl ? a.ctl->it + 1 : 0));
+  if (a.ctl && !(ctl_pass_active(a.ctl) && a.ctl->converge)) return;   // (the exact kernel skips the same passes)
+  const int n = a.ctl ? a.ctl->n : a.n;
+  if ((int)blockIdx.x * STENCIL_THREADS >= n) return;   // a CTA without queries is not counted in stencil_done
+  const int i = blockIdx.x * STENCIL_THREADS + tid;
+  if (i < n) stencil_query<K>(a, sm, tid, i);
+  // every query of this CTA is published: count the CTA in; the CTA that completes the count closes the list
+  __syncthreads();
+  int last = 0;
+  if (tid == 0) {
+    const int nq = a.ctl ? a.ctl->n : a.n;   // (read again: keeps the search's register budget as it was)
+    last = atom_add_release(a.stencil_done, 1) == (nq + STENCIL_THREADS - 1) / STENCIL_THREADS - 1;
+    if (last) __threadfence();   // (acquire: every other CTA's entries, hence the final work_count, happened before)
+  }
+  if (__syncthreads_or(last)) {
+    const int nw = ld_relaxed(a.work_count);
+    // (no data behind WORK_END: relaxed stores, a release would put a GPU-wide memory barrier before each one)
+    for (int j = tid; j < a.exact_warps; j += STENCIL_THREADS) st_relaxed(&a.worklist[nw + j], WORK_END);
   }
   FLB_TRACE_END(2 * 8 + (a.ctl ? a.ctl->it + 1 : 0));
 }

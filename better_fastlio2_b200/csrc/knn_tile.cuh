@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(TILE_THREADS, 3) k_knn_tile(KnnArgs a) {
     a.nbr[(size_t)r * a.stride + i] = o;
   }
   a.cnt[i] = (unsigned char)c;
-  if (!done) a.worklist[atomicAdd(a.work_count, 1)] = i;
+  if (!done) st_release(&a.worklist[atomicAdd(a.work_count, 1)], i);   // (published as k_knn_stencil does)
 }
 
 }  // namespace flb

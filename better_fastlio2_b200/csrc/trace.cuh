@@ -22,7 +22,19 @@ __device__ __forceinline__ void trace_mark(int slot, bool begin) {
     else atomicMax(&g_trace[slot].t1, t);
   }
 }
-constexpr int TRACE_DBG = 64;
+// first block start (begin) or last block end of `slot`, stamped by the calling thread itself
+__device__ __forceinline__ void trace_stamp(int slot, bool begin) {
+  const unsigned long long t = gtimer();
+  if (begin) atomicMin(&g_trace[slot].t0, t);
+  else atomicMax(&g_trace[slot].t1, t);
+}
+// 4-us bucket (0..15) of the time elapsed since the earliest block start recorded in `slot`
+__device__ __forceinline__ int trace_bucket_since(int slot) {
+  const unsigned long long t0 = *(volatile unsigned long long*)&g_trace[slot].t0;
+  const unsigned long long t = gtimer();
+  return t > t0 ? (int)min((t - t0) / 4000ull, 15ull) : 0;
+}
+constexpr int TRACE_DBG = 128;
 __device__ unsigned long long g_dbg[TRACE_DBG];
 __device__ __forceinline__ void dbg_add(int idx, unsigned long long v) { atomicAdd(&g_dbg[idx], v); }
 __device__ __forceinline__ void dbg_max(int idx, unsigned long long v) { atomicMax(&g_dbg[idx], v); }
@@ -36,6 +48,8 @@ __device__ __forceinline__ void trace_phase(int idx) {
 #define FLB_DBG_ADD(idx, v) flb::dbg_add((idx), (unsigned long long)(v))
 #define FLB_DBG_MAX(idx, v) flb::dbg_max((idx), (unsigned long long)(v))
 #define FLB_DBG_CLOCK(var) const long long var = clock64()
+#define FLB_TRACE_STAMP(slot, begin) flb::trace_stamp((slot), (begin))
+#define FLB_TRACE_HIST(idx0, slot) flb::dbg_add((idx0) + flb::trace_bucket_since(slot), 1)
 #else
 #define FLB_TRACE_BEGIN(slot)
 #define FLB_TRACE_END(slot)
@@ -43,4 +57,6 @@ __device__ __forceinline__ void trace_phase(int idx) {
 #define FLB_DBG_ADD(idx, v)
 #define FLB_DBG_MAX(idx, v)
 #define FLB_DBG_CLOCK(var)
+#define FLB_TRACE_STAMP(slot, begin)
+#define FLB_TRACE_HIST(idx0, slot)
 #endif

@@ -40,9 +40,31 @@ __device__ __forceinline__ unsigned long long global_timer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_sync() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl_wait();
+  pdl_trigger();
+}
+// GPU-scope memory operations of a producer kernel handing data to a consumer kernel running beside it.  An acquire
+// (ld.acquire, or a fence after a relaxed read) invalidates the SM's whole L1 (CCTL.IVALL), which the other kernel's
+// warps on that SM depend on: poll with relaxed loads and acquire once, when the awaited value has arrived.
+__device__ __forceinline__ void st_release(int* p, int v) { asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ void st_relaxed(int* p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ int ld_relaxed(const int* p) {
+  int v;
+  asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ int ld_acquire(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ int atom_add_release(int* p, int v) {
+  int old;
+  asm volatile("atom.release.gpu.global.add.s32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
+  return old;
 }
 
 constexpr uint64_t KEY_EMPTY = 0xFFFFFFFFFFFFFFFFull;
@@ -67,7 +89,8 @@ enum Counter : int {
   CNT_CMAX_X, CNT_CMAX_Y, CNT_CMAX_Z,
   CNT_COUNT = 32
 };
-enum DevError : int { ERR_BLOCKS_FULL = 1, ERR_OVF_FULL = 2, ERR_HASH_FULL = 4, ERR_COARSE_FULL = 8, ERR_RANGE = 16 };
+// ERR_KNN_STALL: the exact k-NN kernel gave up waiting for its work list (a broken hand-over protocol; never expected)
+enum DevError : int { ERR_BLOCKS_FULL = 1, ERR_OVF_FULL = 2, ERR_HASH_FULL = 4, ERR_COARSE_FULL = 8, ERR_RANGE = 16, ERR_KNN_STALL = 32 };
 
 // one hash entry = one 32-byte sector: key, block index and the block's voxel-occupancy word side by side
 struct __align__(32) HEntry {

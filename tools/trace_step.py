@@ -3,8 +3,9 @@
 
   FLB_LIB=better_fastlio2_b200/libfastlio_b200_trace.so python tools/trace_step.py [--steps 20] [--out file.json]
 
-Prints, per kernel and pass, the mean start / end (us after k_esikf_begin started) over the steps, and the clock-cycle
-phases inside k_esikf_post.  The timeline comes from %globaltimer stamps taken by the kernels themselves, so it shows
+Prints, per kernel and pass, the mean start / end (us after k_esikf_begin started) over the steps, the clock-cycle
+phases inside k_esikf_post, and when the first pass's unresolved k-NN queries are published by the stencil kernel and
+picked up by the exact kernel.  The timeline comes from %globaltimer stamps taken by the kernels themselves, so it shows
 the real critical path of the CUDA-graph execution (launch gaps, side-stream overlap) without a profiler attached.
 """
 import argparse
@@ -19,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
-NAMES = {0: "esikf_begin", 1: "esikf_pre", 2: "knn_stencil", 3: "knn_exact", 4: "residual", 5: "esikf_post", 6: "classify",
+NAMES = {0: "esikf_begin", 1: "esikf_pre", 2: "knn_stencil", 3: "knn_exact_pick", 4: "residual", 5: "esikf_post", 6: "classify",
          7: "touch_blocks", 8: "ds_scatter", 9: "ds_apply", 10: "append_points", 11: "relocate_chains"}
 PHASES = ["start", "partials reduced", "matrices staged", "inverse", "gain+dx", "boxplus(+J)", "cov/state written"]
 
@@ -52,9 +53,9 @@ def main():
     NS, NP = 128, 96
     tr = (C.c_ulonglong * (2 * NS))()
     ph = (C.c_longlong * NP)()
-    dbg = (C.c_ulonglong * 64)()
-    dbg_sum = np.zeros(64, np.float64)
-    dbg_max = np.zeros(64, np.float64)
+    dbg = (C.c_ulonglong * 128)()
+    dbg_sum = np.zeros(128, np.float64)
+    dbg_max = np.zeros(128, np.float64)
 
     def step(k):
         ses.scan_set_device(dev[k].data_ptr(), len(work["scans"][k]))
@@ -96,6 +97,8 @@ def main():
                 phases.setdefault(pas, []).append([(p[pas, j] - p[pas, 0]) if p[pas, j] else -1 for j in range(7)])
     out = {"steps": args.steps, "timeline_us": [], "post_phases_cycles": {}, "last_kernel_end_us_mean": float(np.mean(total))}
     print(f"# mean over {args.steps} steps; us after k_esikf_begin started; last kernel end {np.mean(total):.1f} us")
+    print("# knn_exact_pick: the exact k-NN kernel runs beside the stencil kernel; start = its first work-list pick-up, "
+          "end = its last warp's exit")
     print(f"{'kernel':<16}{'pass':>5}{'start':>10}{'end':>10}{'dur':>9}{'ran':>6}")
     for slot in sorted(rows, key=lambda s: np.mean([r[0] for r in rows[s]])):
         r = np.array(rows[slot])
@@ -135,6 +138,12 @@ def main():
               f"{dbg_sum[45] / max(dbg_sum[43], 1):.1f} such lanes each); largest per-lane candidate count of a warp: mean={dbg_sum[56] / nw:.1f} max={dbg_max[57]:.0f}")
         print("# stencil kernel, first pass: share of warps by duration (8192-cycle buckets): " +
               " ".join(f"{dbg_sum[48 + j] / nw:.3f}" for j in range(8)))
+    for nm, i0 in (("published by the stencil kernel", 64), ("picked up by the exact kernel", 80)):
+        h = dbg_sum[i0:i0 + 16]
+        if h.sum() > 0:
+            print(f"# first pass, unresolved queries {nm}: share by us after the stencil kernel's start (4-us buckets, last = 60+): " +
+                  " ".join(f"{v / h.sum():.3f}" for v in h) + f"  ({h.sum() / S:.0f}/step)")
+            out.setdefault("worklist_hist_4us", {})[nm] = (h / S).tolist()
     if args.pairs > 0:
         # two steps in flight: device time from the first kernel of step k to the last kernel of step k+1, against twice the
         # single-step span -> what the device loses BETWEEN two graph launches (copies, graph start-up)
