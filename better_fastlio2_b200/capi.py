@@ -72,6 +72,16 @@ class RawLayout(C.Structure):
                 ("off_time", C.c_int), ("off_ring", C.c_int), ("off_tag", C.c_int), ("off_line", C.c_int)]
 
 
+class IcpConfig(C.Structure):
+    _fields_ = [("max_correspondence_distance", C.c_double), ("max_iterations", C.c_int),
+                ("transformation_epsilon", C.c_double), ("euclidean_fitness_epsilon", C.c_double)]
+
+
+class IcpResult(C.Structure):
+    _fields_ = [("final_transformation", C.c_float * 16), ("converged", C.c_int), ("iterations", C.c_int), ("state", C.c_int),
+                ("n_source", C.c_int), ("n_target", C.c_int), ("n_correspondences", C.c_int), ("fitness_score", C.c_double)]
+
+
 K_CLASSES = ["transform", "knn", "residual", "reduce", "classify", "insert", "delete"]
 
 _lib = None
@@ -95,7 +105,7 @@ EXPORTS = [
     "flb_keyframes_create", "flb_keyframes_destroy", "flb_keyframes_append_frontend", "flb_keyframes_append",
     "flb_keyframes_download", "flb_keyframes_info", "flb_keyframes_size", "flb_map_reconstruct_from_keyframes",
     "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
-    "flb_keyframes_scan_context", "flb_keyframes_scan_contexts",
+    "flb_keyframes_scan_context", "flb_keyframes_scan_contexts", "flb_keyframes_icp",
 ]
 
 
@@ -188,6 +198,8 @@ def lib():
         L.flb_keyframes_assemble.argtypes = [vp, vp, C.c_int, C.c_int, fp, C.c_float, fp, fp, C.c_int, ip]
         L.flb_keyframes_scan_context.argtypes = [vp, vp, C.c_int, C.c_int, fp, C.c_double, dp]
         L.flb_keyframes_scan_contexts.argtypes = [vp, vp, C.c_int, C.c_double, dp]
+        L.flb_keyframes_icp.argtypes = [vp, vp, C.c_int, C.c_int, fp, fp, vp, C.c_int, C.c_int, fp, C.POINTER(IcpConfig),
+                                        C.POINTER(IcpResult), vp, fp]
         _lib = L
     return _lib
 
@@ -670,6 +682,8 @@ def reconstruct_keyframes(tree, clouds48, poses6, leaf):
 
 
 KF_POSE6, KF_AFFINE = 0, 1   # FLB_KF_POSE6 / FLB_KF_AFFINE
+# FLB_ICP_* convergence states
+ICP_STATES = ["NOT_CONVERGED", "ITERATIONS", "TRANSFORM", "ABS_MSE", "REL_MSE", "NO_CORRESPONDENCES"]
 SC_RINGS, SC_SECTORS = 20, 60  # FLB_SC_RINGS / FLB_SC_SECTORS
 
 
@@ -791,6 +805,36 @@ class KeyFrameStore:
         _chk(lib().flb_keyframes_scan_contexts(self.h, _p(ids) if len(ids) else None, len(ids), float(lidar_height),
                                                _p(out) if len(ids) else None))
         return out
+
+    def icp(self, src_ids, tgt_ids, src_poses6=None, src_affines=None, tgt_poses6=None, tgt_affines=None, pre_pose6=None,
+            max_correspondence_distance=200.0, max_iterations=100, transformation_epsilon=1e-6, euclidean_fitness_epsilon=1e-6,
+            correspondences=False):
+        """performLoopClosure's ICP on the device: the dense assembly of src_ids (then moved by pre_pose6, when given) onto
+        the dense assembly of tgt_ids.  Returns a dict (final_transformation (4,4) float32, converged, iterations, state,
+        state_name, n_source, n_target, n_correspondences, fitness_score) and, with correspondences=True, also the last
+        iteration's nearest target index (-1: none) and d² of every source point."""
+        src_ids = np.ascontiguousarray(src_ids, np.int32).reshape(-1)
+        tgt_ids = np.ascontiguousarray(tgt_ids, np.int32).reshape(-1)
+        sk, st = self._transforms(src_ids, src_poses6, src_affines)
+        tk, tt = self._transforms(tgt_ids, tgt_poses6, tgt_affines)
+        pre = None if pre_pose6 is None else np.ascontiguousarray(pre_pose6, np.float32).reshape(6)
+        cfg = IcpConfig(float(max_correspondence_distance), int(max_iterations), float(transformation_epsilon),
+                        float(euclidean_fitness_epsilon))
+        r = IcpResult()
+        idx = d2 = None
+        if correspondences:
+            n = self._selection_size(src_ids)
+            idx = np.empty(max(n, 1), np.int32)
+            d2 = np.empty(max(n, 1), np.float32)
+        _chk(lib().flb_keyframes_icp(self.h, _p(src_ids) if len(src_ids) else None, len(src_ids), sk, _p(st) if len(src_ids) else None,
+                                     _p(pre), _p(tgt_ids) if len(tgt_ids) else None, len(tgt_ids), tk,
+                                     _p(tt) if len(tgt_ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(d2)))
+        res = {"final_transformation": np.array(r.final_transformation[:], np.float32).reshape(4, 4), "converged": bool(r.converged),
+               "iterations": r.iterations, "state": r.state, "state_name": ICP_STATES[r.state], "n_source": r.n_source,
+               "n_target": r.n_target, "n_correspondences": r.n_correspondences, "fitness_score": r.fitness_score}
+        if correspondences:
+            return res, idx[:r.n_source].copy(), d2[:r.n_source].copy()
+        return res
 
 
 def make_fov(cube_len=200.0, det_range=100.0):

@@ -1745,3 +1745,4 @@ extern "C" int flb_debug_trace_read(unsigned long long* out, long long* phases, 
 #include "preprocess_host.cuh"
 #include "keyframe_host.cuh"
 #include "scan_context_host.cuh"
+#include "icp_host.cuh"

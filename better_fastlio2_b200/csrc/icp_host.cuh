@@ -1,0 +1,393 @@
+// icp_host.cuh — performLoopClosure's ICP (laserMapping.cpp:946-974, pcl::IterativeClosestPoint 1.10 with the settings of
+// :947-952 and an identity guess) between two selections of the device key-frame store.  Both sub-maps are assembled by
+// k_kf_assemble into map-side scratch exactly as flb_keyframes_assemble writes them; the source's pre-transform
+// (transformPointCloud(cureKeyframeCloud, &com), :954-962) is one more k_kf_assemble segment over the assembled source.
+// The target index is built once per call; each iteration is one exact 1-NN pass and two fixed-order double reductions
+// on the map stream, one small copy and one synchronisation.  The 3x3 SVD, the 4x4 compositions and the convergence test
+// run here on the host between iterations.  The contract is written out in DESIGN.md §9.  Included after
+// scan_context_host.cuh.
+#pragma once
+#include <cfloat>
+#include <cmath>
+
+#include "icp_kernels.cuh"
+
+// Grow-only ICP scratch, held by the map's KfWork (counted in map_scratch_bytes, freed with the rest of it).
+struct IcpWork {
+  DevBuf<float4> src_raw, src, x, tgt, sorted;   // assembled source, pre-transformed source, input_transformed, target,
+                                                 // sorted finite target (w = original index)
+  DevBuf<unsigned> keys_a, keys_b;               // radix-sort keys
+  DevBuf<int> vals_a, vals_b, order;             // radix-sort values; source visiting order
+  DevBuf<int> corr, open;                        // nearest target per source; open queries of the thread path
+  DevBuf<float> corr_d2;
+  DevBuf<int> cs;                                // CSR cell offsets (n_cells + 1)
+  DevBuf<IcpBox> box;                            // coarse-cell point boxes
+  DevBuf<unsigned char> tmp;                     // CUB temporary storage
+  DevBuf<double> partials;                       // reduction block partials
+  DevBuf<unsigned> misc;                         // bounds keys (6), finite count, open count, reduction counter
+  DevBuf<IcpSums> sums;
+  PinnedBuf<unsigned> h_misc;
+  PinnedBuf<IcpSums> h_sums;
+};
+
+static void icp_release(IcpWork* w) { delete w; }
+
+static size_t icp_device_bytes(const IcpWork* w) {
+  if (!w) return 0;
+  return w->src_raw.cap + w->src.cap + w->x.cap + w->tgt.cap + w->sorted.cap + w->keys_a.cap + w->keys_b.cap + w->vals_a.cap +
+         w->vals_b.cap + w->order.cap + w->corr.cap + w->open.cap + w->corr_d2.cap + w->cs.cap + w->box.cap + w->tmp.cap +
+         w->partials.cap + w->misc.cap + w->sums.cap;
+}
+
+constexpr int ICP_MISC_OPEN = 7, ICP_MISC_COUNTER = 8, ICP_MISC_WORDS = 16;
+constexpr double ICP_CELLS_PER_POINT = 8.0;     // dense fine cells over the target box per finite target point
+constexpr double ICP_MAX_CELLS = 134217728.0;   // 2^27 fine cells (512 MB of offsets) at most
+
+static int icp_work(flb_map* m, IcpWork** out) {
+  if (kf_work(m)) return 1;
+  KfWork& k = *m->kfw;
+  if (!k.icp) {
+    k.icp = new (std::nothrow) IcpWork();
+    if (!k.icp) return set_err("out of host memory");
+  }
+  *out = k.icp;
+  return 0;
+}
+
+// Scratch that follows the sizes of the two selections (the grid's buffers are grown once the grid is known).
+static int icp_scratch(flb_map* m, IcpWork& w, int n_s, int n_t, bool pre) {
+  const size_t ps = sizeof(float4) * (size_t)n_s, pt = sizeof(float4) * (size_t)n_t, is = sizeof(int) * (size_t)n_s;
+  const int nk = std::max(n_s, n_t);
+  const size_t ik = sizeof(int) * (size_t)nk;
+  size_t t1 = 0;
+  CU(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, nk));
+  const int red_blocks = m->sm_count * 2;
+  if (kf_grow(w.src_raw, ps) || (pre && kf_grow(w.src, ps)) || kf_grow(w.x, ps) || kf_grow(w.tgt, pt) || kf_grow(w.sorted, pt) ||
+      kf_grow(w.keys_a, ik) || kf_grow(w.keys_b, ik) || kf_grow(w.vals_a, ik) || kf_grow(w.vals_b, ik) || kf_grow(w.order, is) ||
+      kf_grow(w.corr, is) || kf_grow(w.open, is) || kf_grow(w.corr_d2, sizeof(float) * (size_t)n_s) || kf_grow(w.tmp, t1 + 256) ||
+      grow(w.partials, sizeof(double) * ICP_RED * (size_t)red_blocks, 0) || grow(w.misc, sizeof(unsigned) * ICP_MISC_WORDS, 0) ||
+      grow(w.h_misc, sizeof(unsigned) * ICP_MISC_WORDS, 0) || grow(w.sums, sizeof(IcpSums), 0) || grow(w.h_sums, sizeof(IcpSums), 0))
+    return 1;
+  return 0;
+}
+
+static float icp_fkey(unsigned k) {   // inverse of icp_okey
+  const unsigned u = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
+  float v;
+  memcpy(&v, &u, sizeof(v));
+  return v;
+}
+
+// The grid over the finite target box [lo, hi]: fine edge from the box volume and the point count, at most
+// ICP_MAX_CELLS cells, every axis a multiple of ICP_C.
+static IcpGrid icp_grid(const float* lo, const float* hi, int n_fin) {
+  double ext[3], L = 0.0, amax = 0.0;
+  for (int a = 0; a < 3; ++a) {
+    ext[a] = (double)hi[a] - (double)lo[a];
+    L = std::max(L, ext[a]);
+    amax = std::max(amax, std::max(std::fabs((double)lo[a]), std::fabs((double)hi[a])));
+  }
+  double e = 1.0;
+  if (L > 0.0) {
+    const double floor_e = L / 1024.0;
+    double V = 1.0;
+    for (int a = 0; a < 3; ++a) V *= std::max(ext[a], floor_e);
+    e = std::max(std::cbrt(V / (ICP_CELLS_PER_POINT * n_fin)), floor_e);
+  }
+  IcpGrid g{};
+  for (;;) {
+    int dims[3];
+    double cells = 1.0;
+    for (int a = 0; a < 3; ++a) {
+      dims[a] = ((int)std::floor(ext[a] / e) + 1 + ICP_C - 1) / ICP_C * ICP_C;
+      cells *= dims[a];
+    }
+    if (cells <= ICP_MAX_CELLS) {
+      g.gx = dims[0]; g.gy = dims[1]; g.gz = dims[2];
+      break;
+    }
+    e *= 1.25;
+  }
+  g.ox = lo[0]; g.oy = lo[1]; g.oz = lo[2];
+  g.e = (float)e;
+  g.inv_e = 1.0f / g.e;
+  g.slack = 1e-3f * g.e + 4e-6f * (float)(amax + L);
+  g.cx = g.gx / ICP_C; g.cy = g.gy / ICP_C; g.cz = g.gz / ICP_C;
+  return g;
+}
+
+// ------------------------------------------------------------------------------------------------ host algebra
+// One-sided Jacobi SVD of a 3x3 double matrix: A = U diag(s) V^T, s descending.  Columns of U for a zero singular value
+// are completed to an orthonormal basis (u3 = u1 x u2).
+static void icp_svd3(const double A[9], double U[9], double s[3], double V[9]) {
+  double B[9];
+  memcpy(B, A, sizeof(B));
+  for (int i = 0; i < 9; ++i) V[i] = (i % 4 == 0) ? 1.0 : 0.0;
+  for (int sweep = 0; sweep < 60; ++sweep) {
+    double off = 0.0;
+    for (int p = 0; p < 2; ++p)
+      for (int q = p + 1; q < 3; ++q) {
+        double a = 0, b = 0, c = 0;
+        for (int r = 0; r < 3; ++r) { a += B[3 * r + p] * B[3 * r + p]; b += B[3 * r + q] * B[3 * r + q]; c += B[3 * r + p] * B[3 * r + q]; }
+        if (c == 0.0 || std::fabs(c) <= 1e-300) continue;
+        off = std::max(off, std::fabs(c) / std::sqrt(a * b));
+        const double zeta = (b - a) / (2.0 * c);
+        const double t = (zeta >= 0 ? 1.0 : -1.0) / (std::fabs(zeta) + std::sqrt(1.0 + zeta * zeta));
+        const double cs = 1.0 / std::sqrt(1.0 + t * t), sn = cs * t;
+        for (int r = 0; r < 3; ++r) {
+          const double bp = B[3 * r + p], bq = B[3 * r + q];
+          B[3 * r + p] = cs * bp - sn * bq;
+          B[3 * r + q] = sn * bp + cs * bq;
+          const double vp = V[3 * r + p], vq = V[3 * r + q];
+          V[3 * r + p] = cs * vp - sn * vq;
+          V[3 * r + q] = sn * vp + cs * vq;
+        }
+      }
+    if (!(off > 1e-15)) break;
+  }
+  int ord[3] = {0, 1, 2};
+  double nrm[3];
+  for (int j = 0; j < 3; ++j) nrm[j] = std::sqrt(B[j] * B[j] + B[3 + j] * B[3 + j] + B[6 + j] * B[6 + j]);
+  std::sort(ord, ord + 3, [&](int x, int y) { return nrm[x] > nrm[y]; });
+  double Bs[9], Vs[9];
+  for (int j = 0; j < 3; ++j)
+    for (int r = 0; r < 3; ++r) { Bs[3 * r + j] = B[3 * r + ord[j]]; Vs[3 * r + j] = V[3 * r + ord[j]]; }
+  memcpy(V, Vs, sizeof(Vs));
+  for (int j = 0; j < 3; ++j) s[j] = nrm[ord[j]];
+  const double tiny = std::max(s[0], 1e-300) * 1e-13;
+  for (int j = 0; j < 3; ++j)
+    for (int r = 0; r < 3; ++r) U[3 * r + j] = s[j] > tiny ? Bs[3 * r + j] / s[j] : 0.0;
+  if (!(s[1] > tiny)) {   // rank <= 1: any unit vector orthogonal to u1
+    const double u0[3] = {U[0], U[3], U[6]};
+    double w[3] = {0, 0, 0};
+    w[std::fabs(u0[0]) < 0.6 ? 0 : (std::fabs(u0[1]) < 0.6 ? 1 : 2)] = 1.0;
+    const double d = w[0] * u0[0] + w[1] * u0[1] + w[2] * u0[2];
+    double v[3] = {w[0] - d * u0[0], w[1] - d * u0[1], w[2] - d * u0[2]};
+    const double nv = std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    for (int r = 0; r < 3; ++r) U[3 * r + 1] = v[r] / nv;
+  }
+  if (!(s[2] > tiny)) {
+    U[2] = U[3] * U[7] - U[6] * U[4];
+    U[5] = U[6] * U[1] - U[0] * U[7];
+    U[8] = U[0] * U[4] - U[3] * U[1];
+  }
+}
+
+static double icp_det3(const double M[9]) {
+  return M[0] * (M[4] * M[8] - M[5] * M[7]) - M[1] * (M[3] * M[8] - M[5] * M[6]) + M[2] * (M[3] * M[7] - M[4] * M[6]);
+}
+
+// TransformationEstimationSVD (Umeyama, no scaling) from the sums: H = Σ (t - μt)(s - μs)^T = U S V^T,
+// R = U diag(1, 1, det U det V < 0 ? -1 : 1) V^T, t = μt - R μs, cast to a float row-major 4x4.
+static void icp_rigid(const IcpSums& s, float T[16]) {
+  double U[9], sv[3], V[9], R[9];
+  icp_svd3(s.h, U, sv, V);
+  const double d3 = icp_det3(U) * icp_det3(V) < 0 ? -1.0 : 1.0;
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) R[3 * r + c] = U[3 * r + 0] * V[3 * c + 0] + U[3 * r + 1] * V[3 * c + 1] + d3 * U[3 * r + 2] * V[3 * c + 2];
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) T[4 * r + c] = (float)R[3 * r + c];
+    T[4 * r + 3] = (float)(s.mu_t[r] - (R[3 * r] * s.mu_s[0] + R[3 * r + 1] * s.mu_s[1] + R[3 * r + 2] * s.mu_s[2]));
+  }
+  T[12] = T[13] = T[14] = 0.f;
+  T[15] = 1.f;
+}
+
+// C = A * B in float, each entry ((a0 b0 + a1 b1) + a2 b2) + a3 b3 (final_transformation_ = transformation_ * final_).
+static void icp_mul4(const float A[16], const float B[16], float C[16]) {
+  float o[16];
+  for (int r = 0; r < 4; ++r)
+    for (int c = 0; c < 4; ++c) {
+      volatile float acc = A[4 * r] * B[c];   // volatile: no contraction or reassociation by the host compiler
+      acc = acc + A[4 * r + 1] * B[4 + c];
+      acc = acc + A[4 * r + 2] * B[8 + c];
+      acc = acc + A[4 * r + 3] * B[12 + c];
+      o[4 * r + c] = acc;
+    }
+  memcpy(C, o, sizeof(o));
+}
+
+static IcpXf icp_xf(const float T[16], bool apply) {
+  IcpXf x{};
+  for (int i = 0; i < 12; ++i) x.m[i] = T[i];
+  x.apply = apply ? 1 : 0;
+  return x;
+}
+
+// DefaultConvergenceCriteria::hasConverged with max_iterations_similar_transforms_ = 0, after ++nr_iterations, on the
+// increment T and the pairs found before it.  Returns the state (FLB_ICP_NOT_CONVERGED: go on); updates *prev_mse.
+static int icp_converged(const flb_icp_config& cfg, int iterations, const float T[16], double n, double sum_d2, double* prev_mse) {
+  if (iterations >= cfg.max_iterations) return FLB_ICP_ITERATIONS;
+  const double cos_angle = 0.5 * ((double)T[0] + (double)T[5] + (double)T[10] - 1.0);
+  const double tr2 = (double)T[3] * (double)T[3] + (double)T[7] * (double)T[7] + (double)T[11] * (double)T[11];
+  if (cos_angle >= 1.0 - cfg.transformation_epsilon && tr2 <= cfg.transformation_epsilon) return FLB_ICP_TRANSFORM;
+  const double mse = sum_d2 / n;
+  if (std::fabs(mse - *prev_mse) < 1e-12) return FLB_ICP_ABS_MSE;
+  if (std::fabs(mse - *prev_mse) / *prev_mse < cfg.euclidean_fitness_epsilon) return FLB_ICP_REL_MSE;
+  *prev_mse = mse;
+  return FLB_ICP_NOT_CONVERGED;
+}
+
+// ------------------------------------------------------------------------------------------------ device passes
+// One exact 1-NN pass: q = xf(in[i]) into w.x, nearest target into w.corr / w.corr_d2.
+static int icp_nn(flb_map* m, IcpWork& w, const IcpGrid& g, const IcpXf& xf, const float4* in, int n_s) {
+  unsigned* open_n = w.misc.p + ICP_MISC_OPEN;
+  CU(cudaMemsetAsync(open_n, 0, sizeof(unsigned), m->stream));
+  k_icp_nn<<<grid_for(n_s, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, xf, w.order.p, n_s, in, w.x.p, w.sorted.p, w.cs.p, w.corr.p,
+                                                                      w.corr_d2.p, w.open.p, (int*)open_n);
+  k_icp_nn_far<<<m->sm_count * 8, 256, 0, m->stream>>>(g, w.open.p, (const int*)open_n, w.x.p, w.sorted.p, w.cs.p, w.box.p, w.corr.p,
+                                                       w.corr_d2.p);
+  m->launches += 2;
+  CU(cudaGetLastError());
+  return 0;
+}
+
+// Both reductions over the pairs of the last pass and the copy of their record; the caller synchronises.
+static int icp_reduce(flb_map* m, IcpWork& w, int n_s, double max_d2, bool cross) {
+  unsigned* counter = w.misc.p + ICP_MISC_COUNTER;
+  const int blocks = m->sm_count * 2;
+  for (int phase = 0; phase < (cross ? 2 : 1); ++phase) {
+    k_icp_reduce<<<blocks, 256, 0, m->stream>>>(phase, n_s, w.corr.p, w.corr_d2.p, w.x.p, w.tgt.p, max_d2, w.partials.p, counter,
+                                                w.sums.p);
+    m->launches++;
+  }
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(w.h_sums.p, w.sums.p, sizeof(IcpSums), cudaMemcpyDeviceToHost, m->stream));
+  return 0;
+}
+
+static void icp_no_pairs(int n_s, int* out_idx, float* out_d2) {
+  for (int i = 0; i < n_s; ++i) {
+    if (out_idx) out_idx[i] = -1;
+    if (out_d2) out_d2[i] = INFINITY;
+  }
+}
+
+static bool icp_cfg_ok(const flb_icp_config* c) {
+  return std::isfinite(c->max_correspondence_distance) && std::isfinite(c->transformation_epsilon) &&
+         std::isfinite(c->euclidean_fitness_epsilon) && c->max_iterations >= 0 && c->max_correspondence_distance >= 0;
+}
+
+extern "C" int flb_keyframes_icp(flb_keyframes* k, const int* src_ids, int n_src, int src_kind, const float* src_transforms,
+                                 const float* src_pre_pose6, const int* tgt_ids, int n_tgt, int tgt_kind, const float* tgt_transforms,
+                                 const flb_icp_config* cfg, flb_icp_result* out, int* out_corr_index, float* out_corr_d2) {
+  const char* who = "flb_keyframes_icp";
+  if (!out) return set_err("%s: null result", who);
+  if (!cfg) return set_err("%s: null config", who);
+  if (!icp_cfg_ok(cfg))
+    return set_err("%s: config values must be finite, max_iterations >= 0 and max_correspondence_distance >= 0", who);
+  if (n_src < 0 || n_tgt < 0) return set_err("%s: negative n_src or n_tgt", who);
+  if ((n_src > 0 && (!src_ids || !src_transforms)) || (n_tgt > 0 && (!tgt_ids || !tgt_transforms)))
+    return set_err("%s: null ids or transforms", who);
+  for (int kind : {src_kind, tgt_kind})
+    if (kind != FLB_KF_POSE6 && kind != FLB_KF_AFFINE)
+      return set_err("%s: transform kinds must be FLB_KF_POSE6 (%d) or FLB_KF_AFFINE (%d)", who, FLB_KF_POSE6, FLB_KF_AFFINE);
+  if (!k) return set_err("%s: null key-frame store", who);
+  int n_s = 0, n_t = 0;
+  if (kf_selection(k, src_ids, n_src, who, &n_s) || kf_selection(k, tgt_ids, n_tgt, who, &n_t)) return 1;
+
+  flb_icp_result res{};
+  for (int i = 0; i < 16; ++i) res.final_transformation[i] = (i % 5 == 0) ? 1.f : 0.f;
+  res.state = FLB_ICP_NOT_CONVERGED;
+  res.n_source = n_s;
+  res.n_target = n_t;
+  res.fitness_score = DBL_MAX;
+  if (n_s == 0 || n_t == 0) {   // initCompute fails: nothing registered
+    icp_no_pairs(n_s, out_corr_index, out_corr_d2);
+    *out = res;
+    return 0;
+  }
+  flb_map* m = k->map;
+  CU(cudaSetDevice(m->cfg.device));
+  IcpWork* wp = nullptr;
+  if (icp_work(m, &wp) || icp_scratch(m, *wp, n_s, n_t, src_pre_pose6 != nullptr)) return 1;
+  IcpWork& w = *wp;
+
+  // the two loop sub-maps (loopFindNearKeyframes, :918-920), then cureKeyframeCloud = transformPointCloud(.., &com)
+  std::vector<KfSeg> segs;
+  kf_selection_segs(k, tgt_ids, n_tgt, tgt_kind, tgt_transforms, segs);
+  if (kf_assemble_enqueue(m, segs, k->xyzi, nullptr, n_t, w.tgt.p, nullptr)) return 1;
+  kf_selection_segs(k, src_ids, n_src, src_kind, src_transforms, segs);
+  if (kf_assemble_enqueue(m, segs, k->xyzi, nullptr, n_s, w.src_raw.p, nullptr)) return 1;
+  const float4* S = w.src_raw.p;
+  if (src_pre_pose6) {
+    const std::vector<KfSeg> pre{kf_seg(affine_from_rpy(src_pre_pose6).t, false, 0, 0, n_s)};
+    if (kf_assemble_enqueue(m, pre, w.src_raw.p, nullptr, n_s, w.src.p, nullptr)) return 1;
+    S = w.src.p;
+  }
+
+  // the target's finite box and count
+  const unsigned init[ICP_MISC_WORDS] = {~0u, ~0u, ~0u};
+  memcpy(w.h_misc.p, init, sizeof(init));
+  CU(cudaMemcpyAsync(w.misc.p, w.h_misc.p, sizeof(init), cudaMemcpyHostToDevice, m->stream));
+  k_icp_bounds<<<grid_for(n_t, 256, m->sm_count * 4), 256, 0, m->stream>>>(w.tgt.p, n_t, w.misc.p);
+  m->launches++;
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(w.h_misc.p, w.misc.p, sizeof(unsigned) * 7, cudaMemcpyDeviceToHost, m->stream));
+  CU(cudaStreamSynchronize(m->stream));
+  const int n_fin = (int)w.h_misc.p[6];
+  if (n_fin == 0) {   // every target point dropped by KdTreeFLANN: initCompute fails
+    icp_no_pairs(n_s, out_corr_index, out_corr_d2);
+    *out = res;
+    return 0;
+  }
+  float lo[3], hi[3];
+  for (int a = 0; a < 3; ++a) { lo[a] = icp_fkey(w.h_misc.p[a]); hi[a] = icp_fkey(w.h_misc.p[3 + a]); }
+  const IcpGrid g = icp_grid(lo, hi, n_fin);
+  const unsigned n_cells = (unsigned)g.gx * g.gy * g.gz;
+  const int n_coarse = g.cx * g.cy * g.cz;
+  if (grow(w.cs, sizeof(int) * ((size_t)n_cells + 1), 0) || grow(w.box, sizeof(IcpBox) * (size_t)n_coarse, 0)) return 1;
+
+  // the index: finite target points sorted by cell, CSR offsets, coarse boxes; the source's visiting order
+  const int gt = grid_for(n_t, 256, m->sm_count * 8), gs = grid_for(n_s, 256, m->sm_count * 8);
+  size_t tb = w.tmp.cap;
+  k_icp_keys<<<gt, 256, 0, m->stream>>>(g, w.tgt.p, n_t, w.keys_a.p, w.vals_a.p);
+  CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)w.keys_a.p, w.keys_b.p, (const int*)w.vals_a.p, w.vals_b.p, n_t, 0, 32,
+                                     m->stream));
+  k_icp_gather<<<grid_for(n_fin, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.vals_b.p, w.tgt.p, n_fin, w.sorted.p);
+  k_icp_cell_start<<<grid_for(n_fin + 1, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.keys_b.p, n_fin, n_cells, w.cs.p);
+  k_icp_coarse_boxes<<<grid_for(n_coarse, 8, m->sm_count * 8), 256, 0, m->stream>>>(w.sorted.p, w.cs.p, n_coarse, w.box.p);
+  k_icp_keys<<<gs, 256, 0, m->stream>>>(g, S, n_s, w.keys_a.p, w.vals_a.p);
+  tb = w.tmp.cap;
+  CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)w.keys_a.p, w.keys_b.p, (const int*)w.vals_a.p, w.order.p, n_s, 0, 32,
+                                     m->stream));
+  m->launches += 6 + 2 * 5;   // + the radix sorts' kernels
+  CU(cudaGetLastError());
+
+  // the iterations (icp.hpp computeTransformation)
+  const double max_d2 = cfg->max_correspondence_distance * cfg->max_correspondence_distance;
+  float T[16], final_T[16];
+  memcpy(final_T, res.final_transformation, sizeof(final_T));
+  memcpy(T, final_T, sizeof(T));
+  double prev_mse = DBL_MAX;
+  for (int it = 0;; ++it) {
+    // input_transformed <- T_{k-1} * input_transformed, fused into the pass (iteration 0 reads the source itself)
+    if (icp_nn(m, w, g, icp_xf(T, it > 0), it == 0 ? S : w.x.p, n_s) || icp_reduce(m, w, n_s, max_d2, true)) return 1;
+    CU(cudaStreamSynchronize(m->stream));
+    const IcpSums sm = *w.h_sums.p;
+    res.n_correspondences = (int)sm.n;
+    if (sm.n < 3) {   // min_number_correspondences_
+      res.state = FLB_ICP_NO_CORRESPONDENCES;
+      break;
+    }
+    icp_rigid(sm, T);
+    icp_mul4(T, final_T, final_T);
+    res.iterations = it + 1;
+    res.state = icp_converged(*cfg, res.iterations, T, sm.n, sm.d2, &prev_mse);
+    if (res.state != FLB_ICP_NOT_CONVERGED) {
+      res.converged = 1;
+      break;
+    }
+  }
+  memcpy(res.final_transformation, final_T, sizeof(final_T));
+  if (out_corr_index) CU(cudaMemcpyAsync(out_corr_index, w.corr.p, sizeof(int) * (size_t)n_s, cudaMemcpyDeviceToHost, m->stream));
+  if (out_corr_d2) CU(cudaMemcpyAsync(out_corr_d2, w.corr_d2.p, sizeof(float) * (size_t)n_s, cudaMemcpyDeviceToHost, m->stream));
+
+  // getFitnessScore(): the original source transformed once by final, every finite point's nearest d², no cut
+  if (icp_nn(m, w, g, icp_xf(final_T, true), S, n_s) || icp_reduce(m, w, n_s, DBL_MAX, false)) return 1;
+  CU(cudaStreamSynchronize(m->stream));
+  const IcpSums fs = *w.h_sums.p;
+  res.fitness_score = fs.n > 0 ? fs.d2 / fs.n : DBL_MAX;
+  *out = res;
+  return 0;
+}

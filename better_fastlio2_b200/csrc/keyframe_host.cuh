@@ -7,6 +7,10 @@
 #include "keyframe_kernels.cuh"
 #include "scan_context_kernels.cuh"
 
+struct IcpWork;                            // ICP scratch (icp_host.cuh)
+static void icp_release(IcpWork* w);
+static size_t icp_device_bytes(const IcpWork* w);
+
 // ------------------------------------------------------------------------------------------------ map-side scratch
 // Kept with the map and only ever grown, like kf_raw / kf_in / kf_out: the readers run every kd_step key frames or on a
 // service call with selections of similar size, and cudaMalloc / cudaFree of a few hundred MB cost more than the kernels.
@@ -22,11 +26,13 @@ struct KfWork {
   PinnedBuf<ScChunk> h_chunk;                  //   and its staging
   DevBuf<unsigned> d_sc_keys;                  // Scan Context keys, SC_BINS per descriptor
   PinnedBuf<unsigned> h_sc_keys;               //   and their staging
+  IcpWork* icp = nullptr;                      // flb_keyframes_icp's sub-maps, target index and reductions
 };
 
 static void kfw_release(KfWork* w) {
   if (!w) return;
   if (w->ev_seg) Q(cudaEventDestroy(w->ev_seg));
+  icp_release(w->icp);
   delete w;
 }
 
@@ -63,7 +69,7 @@ static int kf_scratch(flb_map* m, int n, bool curv, bool filter) {
 static long long kf_scratch_bytes(const flb_map* m) {
   size_t b = m->kf_raw.cap + m->kf_in.cap + m->kf_out.cap;   // device bytes (the pinned staging is not counted)
   if (const KfWork* w = m->kfw)
-    b += w->cin.cap + w->cout.cap + w->d_seg.cap + w->d_chunk.cap + w->d_sc_keys.cap + vg_device_bytes(w->vg);
+    b += w->cin.cap + w->cout.cap + w->d_seg.cap + w->d_chunk.cap + w->d_sc_keys.cap + vg_device_bytes(w->vg) + icp_device_bytes(w->icp);
   return (long long)b;
 }
 

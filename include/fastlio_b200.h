@@ -412,6 +412,47 @@ int flb_keyframes_scan_context(flb_keyframes* kf, const int* ids, int n_ids, int
  * out_descs = n_ids x 20 x 60 doubles; an empty key frame gives all zeros. */
 int flb_keyframes_scan_contexts(flb_keyframes* kf, const int* ids, int n_ids, double lidar_height, double* out_descs);
 
+/* ------------------------------------------------------------------------------------------------ loop registration
+ * performLoopClosure's ICP (laserMapping.cpp:946-974): pcl::IterativeClosestPoint<PointType, PointType> (PCL 1.10) with an
+ * identity guess, between the two dense loop sub-maps of the store, computed where they are; no cloud is downloaded.
+ * Source = the dense assembly of (src_ids, src_transforms), then transformPointCloud(.., pose6 src_pre_pose6) when it is
+ * not NULL (the Scan Context yaw `com`, :954-962); target = the dense assembly of (tgt_ids, tgt_transforms); both as
+ * flb_keyframes_assemble writes them.  A point's index is its position in the assembled cloud.  Each iteration pairs every
+ * finite source point with its exact nearest finite target point (float d² = (dx*dx + dy*dy) + dz*dz; equal d²: the lower
+ * target index), keeps the pairs with d² <= max_correspondence_distance² (in double), stops with NO_CORRESPONDENCES below 3
+ * pairs, fits R, t by Umeyama (SVD of the cross-covariance, reflection-corrected; sums in double, fixed order), applies
+ * the float increment to the source and to the final transformation and runs the DefaultConvergenceCriteria tests.
+ * fitness_score is getFitnessScore(): the mean nearest d² of the original source moved once by the final transformation.
+ * DESIGN.md §9 states the contract and its deviations from PCL.  Every argument is checked before any device work; one
+ * synchronisation per iteration; the store and the map are not modified.  The sub-maps, the target index and the
+ * reduction buffers are map-side key-frame scratch (flb_keyframes_info, flb_map_release_keyframe_scratch). */
+#define FLB_ICP_NOT_CONVERGED 0      /* CONVERGENCE_CRITERIA_NOT_CONVERGED (also: empty source or target) */
+#define FLB_ICP_ITERATIONS 1         /* nr_iterations >= max_iterations */
+#define FLB_ICP_TRANSFORM 2          /* the increment is within transformation_epsilon */
+#define FLB_ICP_ABS_MSE 3            /* |mse - previous mse| < 1e-12 */
+#define FLB_ICP_REL_MSE 4            /* |mse - previous mse| / previous mse < euclidean_fitness_epsilon */
+#define FLB_ICP_NO_CORRESPONDENCES 5 /* fewer than 3 pairs: not converged, the transformation so far is kept */
+typedef struct flb_icp_config {
+  double max_correspondence_distance;  /* setMaxCorrespondenceDistance (200, laserMapping.cpp:948) */
+  int max_iterations;                  /* setMaximumIterations (100, :949) */
+  double transformation_epsilon;       /* setTransformationEpsilon (1e-6, :950) */
+  double euclidean_fitness_epsilon;    /* setEuclideanFitnessEpsilon (1e-6, :951) */
+} flb_icp_config;
+typedef struct flb_icp_result {
+  float final_transformation[16];      /* getFinalTransformation(), row-major 4x4 */
+  int converged;                       /* hasConverged() */
+  int iterations, state;               /* nr_iterations_; FLB_ICP_* */
+  int n_source, n_target, n_correspondences;   /* assembled sizes; pairs of the last iteration */
+  double fitness_score;                /* getFitnessScore(); DBL_MAX when no point counts */
+} flb_icp_result;
+/* Registers the source selection onto the target selection.  Empty source or target (after dropping non-finite target
+ * points): not converged, 0 iterations, identity, fitness DBL_MAX.  out_corr_index / out_corr_d2 (optional, n_source
+ * entries each) receive the last iteration's nearest target index and its d² for every source point, before the distance
+ * cut (-1 and +inf for a non-finite source point or when nothing was registered). */
+int flb_keyframes_icp(flb_keyframes* kf, const int* src_ids, int n_src, int src_kind, const float* src_transforms,
+                      const float* src_pre_pose6, const int* tgt_ids, int n_tgt, int tgt_kind, const float* tgt_transforms,
+                      const flb_icp_config* cfg, flb_icp_result* out, int* out_corr_index, float* out_corr_d2);
+
 /* Stream access for callers that overlap work (returns a cudaStream_t as void*). */
 void* flb_session_stream(flb_session* s);
 int flb_session_sync(flb_session* s);

@@ -16,6 +16,9 @@
 //   keyframes.scan_context(ids, finalTrans, scLoop.LIDAR_HEIGHT, cureKeyframeSC);
 //   // every key frame's descriptor for the saver (:2504-2505), then scLoop.saveScancontextAndKeys(descs[i])
 //   keyframes.scan_contexts(all_ids, scLoop.LIDAR_HEIGHT, descs);
+//   // the ICP of performLoopClosure (:946-974) once the gate passed: the same selections, com = the SC yaw pose
+//   flb::IcpParams icp;  icp.setMaxCorrespondenceDistance(200); ...;  flb::IcpResult reg;
+//   keyframes.icp(curIds, curT, com, preIds, preT, icp, reg);  reg.hasConverged(), reg.getFitnessScore(), ...
 //
 // Poses6D is anything with points[k].{x, y, z, roll, pitch, yaw} (pcl::PointCloud<PointTypePose>); an affine is
 // anything with operator()(row, col) (Eigen::Affine3f).  Clouds come back with x, y, z, intensity and curvature set
@@ -32,6 +35,30 @@
 #include "scan_frontend_facade.hpp"
 
 namespace flb {
+
+// The five setters of pcl::IterativeClosestPoint that performLoopClosure calls (:947-952), with its values as defaults.
+struct IcpParams {
+  flb_icp_config cfg{200.0, 100, 1e-6, 1e-6};
+  int ransac_iterations = 0;
+  void setMaxCorrespondenceDistance(double d) { cfg.max_correspondence_distance = d; }
+  void setMaximumIterations(int n) { cfg.max_iterations = n; }
+  void setTransformationEpsilon(double e) { cfg.transformation_epsilon = e; }
+  void setEuclideanFitnessEpsilon(double e) { cfg.euclidean_fitness_epsilon = e; }
+  void setRANSACIterations(int n) { ransac_iterations = n; }   // only 0, the reference's value, is accepted
+};
+
+// The three getters the node reads after icp.align(..) (:966-987).
+struct IcpResult {
+  flb_icp_result r{};
+  bool hasConverged() const { return r.converged != 0; }
+  double getFitnessScore() const { return r.fitness_score; }
+  // into anything with operator()(row, col) of a 4x4, i.e. Eigen::Matrix4f (correctionLidarFrame.matrix())
+  template <class M>
+  void getFinalTransformation(M& T) const {
+    for (int i = 0; i < 4; ++i)
+      for (int j = 0; j < 4; ++j) T(i, j) = r.final_transformation[4 * i + j];
+  }
+};
 
 class KeyFrameStore {
  public:
@@ -130,6 +157,26 @@ class KeyFrameStore {
     descs.resize(ids.size());
     for (size_t j = 0; j < ids.size(); ++j) to_mat(&sc_[j * kScBins], descs[j]);
     return true;
+  }
+
+  // performLoopClosure's ICP (:946-974) on the device: the loop sub-map of (curIds, curT) moved by the pose `com`
+  // (transformPointCloud(cureKeyframeCloud, &com), :954-962) registered onto the loop sub-map of (preIds, preT), with the
+  // same ids and affines as the Scan Context gate.  No cloud is assembled on the host or downloaded.  com is anything
+  // with x, y, z, roll, pitch, yaw (PointTypePose).
+  template <class Affine, class Alloc, class Pose>
+  bool icp(const std::vector<int>& curIds, const std::vector<Affine, Alloc>& curT, const Pose& com, const std::vector<int>& preIds,
+           const std::vector<Affine, Alloc>& preT, const IcpParams& params, IcpResult& result) {
+    result = IcpResult();
+    if (curT.size() != curIds.size() || preT.size() != preIds.size()) return ok(1, "icp: one affine per key frame");
+    if (params.ransac_iterations != 0) {
+      std::fprintf(stderr, "[fastlio_b200] KeyFrameStore::icp: RANSAC rejection is not offered (setRANSACIterations(0))\n");
+      return false;
+    }
+    const float pre[6] = {com.x, com.y, com.z, com.roll, com.pitch, com.yaw};
+    const std::vector<float> a = affines12(curT), b = affines12(preT);
+    return ok(flb_keyframes_icp(kf_, curIds.data(), (int)curIds.size(), FLB_KF_AFFINE, a.data(), pre, preIds.data(), (int)preIds.size(),
+                                FLB_KF_AFFINE, b.data(), &params.cfg, &result.r, nullptr, nullptr),
+              "icp");
   }
 
   // pcl::copyPointCloud(*surfCloudKeyFrames[k], out)
