@@ -106,6 +106,7 @@ EXPORTS = [
     "flb_keyframes_download", "flb_keyframes_info", "flb_keyframes_size", "flb_map_reconstruct_from_keyframes",
     "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
     "flb_keyframes_scan_context", "flb_keyframes_scan_contexts", "flb_keyframes_icp",
+    "flb_frontend_camera_config", "flb_frontend_camera_image", "flb_frontend_points_colorize", "flb_frontend_points_to_imu",
 ]
 
 
@@ -179,6 +180,10 @@ def lib():
         L.flb_frontend_download_undistorted.argtypes = [vp, fp, fp, vp, C.c_int, ip]
         L.flb_frontend_download_down.argtypes = [vp, fp, fp, C.c_int, ip]
         L.flb_frontend_points_to_world.argtypes = [vp, C.c_int, dp, fp, C.c_int, ip]
+        L.flb_frontend_camera_config.argtypes = [vp, dp, dp, C.c_int, C.c_int]
+        L.flb_frontend_camera_image.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int]
+        L.flb_frontend_points_colorize.argtypes = [vp, C.c_int, dp, fp, vp, C.c_int, ip]
+        L.flb_frontend_points_to_imu.argtypes = [vp, dp, fp, C.c_int, ip]
         L.flb_voxel_grid_filter.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, fp, C.c_int, ip]
         L.flb_frontend_preprocess.argtypes = [vp, C.POINTER(PreprocessConfig), C.POINTER(RawLayout), vp, C.c_int, ip,
                                               C.POINTER(C.c_float)]
@@ -620,6 +625,43 @@ class FrontEnd:
         cnt = C.c_int(0)
         out = np.empty((self.cap, 4), np.float32)
         _chk(lib().flb_frontend_points_to_world(self.h, int(which), _p(st), _p(out), self.cap, C.byref(cnt)))
+        return out[:cnt.value].copy()
+
+    def set_camera(self, cam_ex, cam_in, width=1280, height=720):
+        """paramSetting: cam_ex 16 and cam_in 12 row-major doubles; width x height bounds the image (Wmax x Hmax)."""
+        ex = np.ascontiguousarray(cam_ex, np.float64).reshape(-1)
+        ki = np.ascontiguousarray(cam_in, np.float64).reshape(-1)
+        if ex.size != 16 or ki.size != 12:
+            raise ValueError("cam_ex must hold 16 and cam_in 12 values")
+        _chk(lib().flb_frontend_camera_config(self.h, _p(ex), _p(ki), int(width), int(height)))
+
+    def upload_image(self, img):
+        """imageCallback: img is a (rows, cols, 3) uint8 bgr8 array; rows may be padded (a row stride above 3 * cols)."""
+        a = np.asarray(img)
+        if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+            raise ValueError("image must be a (rows, cols, 3) uint8 array")
+        if a.strides[1:] != (3, 1) or a.strides[0] < 3 * a.shape[1]:
+            a = np.ascontiguousarray(a)
+        _chk(lib().flb_frontend_camera_image(self.h, C.c_void_p(a.ctypes.data), a.shape[0], a.shape[1], a.strides[0]))
+
+    def colorize(self, which, state26, cap=None):
+        """publish_frame_world_color: returns (xyzi (k,4) float32 in the world frame, bgra (k,) uint32 with the bytes
+        b, g, r, a, kept count); k = min(kept count, cap)."""
+        st = np.ascontiguousarray(state26, np.float64)
+        cap = self.cap if cap is None else int(cap)
+        xyzi = np.empty((max(cap, 1), 4), np.float32)
+        bgra = np.empty(max(cap, 1), np.uint32)
+        cnt = C.c_int(0)
+        _chk(lib().flb_frontend_points_colorize(self.h, int(which), _p(st), _p(xyzi), _p(bgra), cap, C.byref(cnt)))
+        k = min(cnt.value, cap)
+        return xyzi[:k].copy(), bgra[:k].copy(), cnt.value
+
+    def to_imu(self, state26):
+        """publish_frame_body: feats_undistort in the IMU frame (x, y, z, intensity)."""
+        st = np.ascontiguousarray(state26, np.float64)
+        cnt = C.c_int(0)
+        out = np.empty((self.cap, 4), np.float32)
+        _chk(lib().flb_frontend_points_to_imu(self.h, _p(st), _p(out), self.cap, C.byref(cnt)))
         return out[:cnt.value].copy()
 
 

@@ -61,6 +61,8 @@ static int vg_enqueue(flb_map* m, VgWork& w, const float4* pts, const float* cur
 // ------------------------------------------------------------------------------------------------ front end object
 struct PpWork;                          // preprocess scratch (preprocess_host.cuh)
 static void pp_release(PpWork* w);
+struct ColorCam;                        // camera state of the colour publisher (color_host.cuh)
+static void cam_release(ColorCam* c);
 struct flb_frontend {
   flb_session* ses = nullptr;
   int cap = 0;
@@ -76,6 +78,7 @@ struct flb_frontend {
   cudaEvent_t ev_poses = nullptr;
   VgWork vg;
   PpWork* pp = nullptr;
+  ColorCam* cam = nullptr;  // null until flb_frontend_camera_config
   bool holds_ref = false;
 };
 
@@ -122,6 +125,7 @@ extern "C" void flb_frontend_destroy(flb_frontend* f) {
   if (f->ev_poses) Q(cudaEventDestroy(f->ev_poses));
   const bool counted = f->holds_ref;
   pp_release(f->pp);
+  cam_release(f->cam);
   delete f;
   if (m && counted) map_release(m);
 }

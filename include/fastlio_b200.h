@@ -285,6 +285,27 @@ int flb_frontend_download_down(flb_frontend* f, float* out_xyzi, float* out_curv
  * feats_down_body (which = 0, dense_pub_en false) or feats_undistort (which = 1) with the posterior state. */
 int flb_frontend_points_to_world(flb_frontend* f, int which, const double* state26, float* out_xyzi, int cap, int* n);
 
+/* Camera colouring of the published scan, publish_frame_world_color (laserMapping.cpp:310-392).
+ * flb_frontend_camera_config is paramSetting (:279-289): cam_ex = 16 row-major doubles (externalMat, 4x4), cam_in = 12
+ * (internalMatProject, 3x4), as read at :2045-2046; width x height bounds the image (the reference's Wmax x Hmax =
+ * 1280 x 720, :232-233).  M = cam_in * cam_ex is formed once, in double.  Configuring zero-fills the device image (the
+ * reference's zero-initialised image_color).  Non-finite parameters and non-positive sizes are rejected. */
+int flb_frontend_camera_config(flb_frontend* f, const double cam_ex[16], const double cam_in[12], int width, int height);
+/* imageCallback (:250-276) after cv_bridge::toCvShare(msg, "bgr8"): copies the top-left height x width window of a
+ * bgr8 image of any row step (step_bytes >= 3 * cols) to the device.  An image smaller than the configured size is
+ * rejected (the reference reads past it). */
+int flb_frontend_camera_image(flb_frontend* f, const unsigned char* bgr8, int rows, int cols, int step_bytes);
+/* The two loops of publish_frame_world_color on feats_down_body (which = 0) or feats_undistort (which = 1): a point is
+ * kept iff its pixel (u, v) = trunc(M*(x,y,z,1) / c2) lies in the image and its lidar-frame x > 0; kept points stay in
+ * cloud order with x,y,z in the world frame (as flb_frontend_points_to_world), the source intensity, and the colour as
+ * one 32-bit word with the bytes b, g, r, a = 255 (PCL_ADD_RGB).  At most cap records are written; *n = the kept count.
+ * DESIGN.md §9 states the contract and its deviations. */
+int flb_frontend_points_colorize(flb_frontend* f, int which, const double* state26, float* out_xyzi, unsigned* out_bgra, int cap,
+                                 int* n);
+/* publish_frame_body (laserMapping.cpp:1543-1558): RGBpointBodyLidarToIMU (:1113-1122), offR * p + offT in double, of
+ * every point of feats_undistort, intensity carried.  At most cap points are written; *n = the cloud size. */
+int flb_frontend_points_to_imu(flb_frontend* f, const double* state26, float* out_xyzi, int cap, int* n);
+
 /* Preprocess::process (src/preprocess.cpp) with feature extraction off (feature_extract_enable, laserMapping.cpp:2040):
  * driver records -> the PointType cloud that becomes meas.lidar, on the device.  Parameters as read at
  * laserMapping.cpp:2034-2041 (preprocess.h:8-14 for the enums):

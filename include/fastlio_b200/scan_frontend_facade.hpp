@@ -9,6 +9,9 @@
 //     its result is ALSO the session's current scan, so LioGpu::begin_scan (the upload) is no longer needed;
 //   * flb::ScanFrontEnd::to_world(...)   replaces the RGBpointBodyToWorld loops of publish_frame_world
 //     (src/laserMapping.cpp:1502-1540);
+//   * flb::ScanFrontEnd::set_camera / upload_image / colorize replace paramSetting, imageCallback and the loops of
+//     publish_frame_world_color (src/laserMapping.cpp:250-392); to_imu(...) replaces the loop of publish_frame_body
+//     (:1543-1558);
 //   * flb::ScanFrontEnd::preprocess(...) replaces Preprocess::process (src/preprocess.cpp, feature extraction off) for a
 //     sensor_msgs::PointCloud2 (Velodyne, Ouster) or livox_ros_driver::CustomMsg: the driver message is uploaded once
 //     and its preprocessed cloud stays on the device as the current scan, which undistort(poses, imu_state) then uses.
@@ -21,8 +24,9 @@
 //
 // Only member names of the reference types are needed (Pose6D: offset_time, acc, gyr, vel, pos, rot —
 // msg/Pose6D.msg; pcl::PointCloud: points; PointType: x,y,z,intensity,curvature; PointCloud2: fields[].name/.offset,
-// point_step, width, height, data; CustomMsg: point_num, points[] with offset_time, x,y,z, reflectivity, tag, line),
-// so the header compiles without ROS/PCL.
+// point_step, width, height, data; CustomMsg: point_num, points[] with offset_time, x,y,z, reflectivity, tag, line;
+// cv::Mat: rows, cols, step[0], data; livox_ros::Point: x,y,z, intensity, b,g,r,a), so the header compiles without
+// ROS/PCL/OpenCV.
 #pragma once
 #include <cstddef>
 #include <cstdio>
@@ -41,6 +45,7 @@ class ScanFrontEnd {
   ~ScanFrontEnd() { if (fe_) flb_frontend_destroy(fe_); }
   bool attach(flb_session* ses, int max_raw_points) {
     if (flb_frontend_create(ses, max_raw_points, &fe_)) { std::fprintf(stderr, "[fastlio_b200] %s\n", flb_last_error()); fe_ = nullptr; return false; }
+    cap_ = max_raw_points;
     return true;
   }
   flb_frontend* handle() { return fe_; }
@@ -170,6 +175,64 @@ class ScanFrontEnd {
     return true;
   }
 
+  // paramSetting (laserMapping.cpp:279-289): cam_ex = 16, cam_in = 12 row-major values (vector<double>, :2045-2046);
+  // width x height bounds the image (the reference's Wmax x Hmax).  Zero-fills the device image.
+  template <class VecEx, class VecIn>
+  bool set_camera(const VecEx& cam_ex, const VecIn& cam_in, int width = 1280, int height = 720) {
+    if (cam_ex.size() < 16 || cam_in.size() < 12) { std::fprintf(stderr, "[fastlio_b200] set_camera: cam_ex needs 16 and cam_in 12 values\n"); return false; }
+    double ex[16], in[12];
+    for (int k = 0; k < 16; ++k) ex[k] = cam_ex[k];
+    for (int k = 0; k < 12; ++k) in[k] = cam_in[k];
+    return ok(flb_frontend_camera_config(fe_, ex, in, width, height), "set_camera");
+  }
+
+  // imageCallback (:250-276): img = cv_bridge::toCvShare(msg, "bgr8")->image (members rows, cols, step[0], data)
+  template <class Mat>
+  bool upload_image(const Mat& img) {
+    return ok(flb_frontend_camera_image(fe_, (const unsigned char*)img.data, (int)img.rows, (int)img.cols, (int)img.step[0]),
+              "upload_image");
+  }
+
+  // The two loops of publish_frame_world_color (:323-381): colorCloud (pcl::PointCloud<livox_ros::Point>) receives the kept
+  // points of feats_undistort (dense_pub_en) or feats_down_body in the world frame, x, y, z, intensity, b, g, r, a set by
+  // member name and every other field zero.
+  template <class State, class Cloud>
+  bool colorize(const State& state_point, bool dense_pub_en, Cloud& colorCloud) {
+    double st[FLB_STATE_DIM];
+    pack_state26(state_point, st);
+    xyzi_.resize((size_t)cap_ * 4 + 4);
+    bgra_.resize((size_t)cap_ + 1);
+    int n = 0;
+    if (!ok(flb_frontend_points_colorize(fe_, dense_pub_en ? 1 : 0, st, xyzi_.data(), bgra_.data(), cap_, &n), "colorize")) return false;
+    if (n > cap_) n = cap_;
+    colorCloud.points.resize(n);
+    for (int i = 0; i < n; ++i) {
+      auto& p = colorCloud.points[i];
+      typedef typename std::remove_reference<decltype(p)>::type P;
+      p = P();
+      const float* v = &xyzi_[4 * (size_t)i];
+      const unsigned c = bgra_[i];
+      p.x = v[0]; p.y = v[1]; p.z = v[2]; p.intensity = v[3];
+      p.b = (unsigned char)(c & 0xFFu); p.g = (unsigned char)((c >> 8) & 0xFFu); p.r = (unsigned char)((c >> 16) & 0xFFu);
+      p.a = (unsigned char)(c >> 24);
+    }
+    return true;
+  }
+
+  // publish_frame_body (:1543-1558): feats_undistort in the IMU frame (RGBpointBodyLidarToIMU), curvature 0
+  template <class State, class Cloud>
+  bool to_imu(const State& state_point, Cloud& laserCloudIMUBody) {
+    double st[FLB_STATE_DIM];
+    pack_state26(state_point, st);
+    xyzi_.resize((size_t)cap_ * 4 + 4);
+    int n = 0;
+    if (!ok(flb_frontend_points_to_imu(fe_, st, xyzi_.data(), cap_, &n), "to_imu")) return false;
+    if (n > cap_) n = cap_;
+    laserCloudIMUBody.points.resize(n);
+    for (int i = 0; i < n; ++i) fill(laserCloudIMUBody.points[i], &xyzi_[4 * (size_t)i], 0.f);
+    return true;
+  }
+
  private:
   int run_preprocess(const flb_preprocess_config& cfg, flb_raw_layout L, const void* rec, int n, float* last_curvature) {
     if (n == 0) L = flb_raw_layout{12, 0, 4, 8, -1, -1, -1, -1, -1};   // nothing to decode; the call still resets the scan
@@ -189,7 +252,9 @@ class ScanFrontEnd {
     return rc == 0;
   }
   flb_frontend* fe_ = nullptr;
+  int cap_ = 0;   // max_raw_points: no cloud of the front end is larger
   std::vector<float> xyzi_, curv_;
+  std::vector<unsigned> bgra_;
 };
 
 // pcl::VoxelGrid<PointT> call shape on top of a ScanFrontEnd.  setInputCloud() is accepted for source compatibility: the
