@@ -271,7 +271,9 @@ extern "C" int flb_map_create(const flb_map_config* cfg, flb_map** out) {
   d.ovf_cap = std::max(1024, m->cfg.max_points / 2);
   // load factor <= 1/4 at full capacity (typically 5-10 % in use): a probe rarely continues past its home slot
   m->hash_cap = next_pow2((uint64_t)d.block_cap * 4);
-  m->chash_cap = next_pow2(std::max<uint64_t>(1024, (uint64_t)d.block_cap / 8));
+  // one coarse cell per block in the worst case (sparse content): with maybe_rehash dropping the cells that deletes emptied,
+  // a map within max_blocks never fills the coarse table (76 B per entry: ckeys + cbits + clist)
+  m->chash_cap = next_pow2(std::max<uint64_t>(1024, (uint64_t)d.block_cap));
   d.hash_mask = m->hash_cap - 1;
   d.chash_mask = m->chash_cap - 1;
   int rc = 0;
@@ -543,25 +545,39 @@ extern "C" int flb_map_delete_points(flb_map* m, const float* xyz, int n, int st
 }
 
 static int maybe_rehash(flb_map* m) {
-  // tombstones only lengthen probe chains; rebuild the key table (16 MB-ish, no point data moves) when they pile up
-  if (m->h_counters[CNT_KEYS_TOMB] <= (int)(m->hash_cap / 8)) return 0;
+  // Tombstones only lengthen probe chains: rebuild the key table (16 MB-ish, no point data moves) when they pile up.
+  // Coarse cells are never removed one by one (coarse_clear only clears a block's bit), so cells that deletes emptied stay
+  // in ckeys and clist until the coarse level is rebuilt from the live blocks.  Between two deletes a cell is created only
+  // together with a new block, so cells - live blocks grows only through deletes, and every delete ends here: keeping
+  // cells <= live blocks + (chash_cap - max_blocks) at this point bounds the cells by chash_cap until the next delete.
+  const int* c = m->h_counters;
+  const int live_blocks = blocks_bumped(m) - c[CNT_BLK_FREE];
+  const bool rehash = c[CNT_KEYS_TOMB] > (int)(m->hash_cap / 8);
+  const bool coarse = c[CNT_COARSE_USED] - live_blocks > (int)m->chash_cap - m->d.block_cap;
+  if (!rehash && !coarse) return 0;
   const int nblk = blocks_bumped(m);
   cudaStream_t st = m->stream;
-  k_rehash_save<<<grid_for(nblk, 256, m->sm_count * 8), 256, 0, st>>>(m->d, nblk);
-  k_hent_clear<<<m->sm_count * 8, 256, 0, st>>>(m->d.hent, m->hash_cap);
-  m->launches += 2;
+  if (rehash) {
+    k_rehash_save<<<grid_for(nblk, 256, m->sm_count * 8), 256, 0, st>>>(m->d, nblk);
+    k_hent_clear<<<m->sm_count * 8, 256, 0, st>>>(m->d.hent, m->hash_cap);
+    m->launches += 2;
+  }
   CU(cudaMemsetAsync(m->d.ckeys, 0xFF, sizeof(uint64_t) * m->chash_cap, st));
   CU(cudaMemsetAsync(m->d.cbits, 0, sizeof(uint64_t) * 8 * (size_t)m->chash_cap, st));
   int init[8] = {0, 0, INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-  // KEYS_TOMB = 0, COARSE_USED = 0, bbox reset
-  CU(cudaMemcpyAsync(m->d.counters + CNT_KEYS_TOMB, &init[0], sizeof(int), cudaMemcpyHostToDevice, st));
+  // KEYS_TOMB = 0 (rehash only), COARSE_USED = 0, bbox reset
+  if (rehash) CU(cudaMemcpyAsync(m->d.counters + CNT_KEYS_TOMB, &init[0], sizeof(int), cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(m->d.counters + CNT_COARSE_USED, &init[1], sizeof(int), cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync(m->d.counters + CNT_CMIN_X, &init[2], sizeof(int) * 6, cudaMemcpyHostToDevice, st));
   CU(cudaStreamSynchronize(st));  // init[] is a stack buffer
-  k_rehash_insert<<<grid_for(nblk, 256, m->sm_count * 8), 256, 0, st>>>(m->d, nblk);
+  if (rehash) {
+    k_rehash_insert<<<grid_for(nblk, 256, m->sm_count * 8), 256, 0, st>>>(m->d, nblk);
+    m->launches++;
+  }
+  k_coarse_rebuild<<<grid_for(nblk, 256, m->sm_count * 8), 256, 0, st>>>(m->d, nblk);
   m->launches++;
   CU(cudaGetLastError());
-  m->rehash_count++;
+  if (rehash) m->rehash_count++;
   return fetch_counters(m);
 }
 

@@ -594,6 +594,14 @@ __global__ void k_rehash_insert(MapDev m, int nblk) {
       if (old == KEY_EMPTY) { m.hent[s].val = (uint32_t)b; m.hent[s].mask = m.brel[b]; m.bslot[b] = s; m.brel[b] = 0ull; break; }
       s = (s + 1) & m.hash_mask;
     }
+  }
+}
+// coarse level rebuild (after its tables were cleared; also the last step of a rehash): every allocated block registers its
+// cell again, so cells that deletes emptied leave ckeys and clist
+__global__ void k_coarse_rebuild(MapDev m, int nblk) {
+  for (int b = blockIdx.x * blockDim.x + threadIdx.x; b < nblk; b += gridDim.x * blockDim.x) {
+    const uint64_t key = m.bkey[b];
+    if (key == KEY_EMPTY) continue;
     int bx, by, bz;
     unpack_key(key, bx, by, bz);
     coarse_set(m, bx, by, bz);

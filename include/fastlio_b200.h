@@ -52,7 +52,9 @@ const char* flb_version(void);
 typedef struct flb_map_config {
   float voxel_size;        /* downsample_size / filter_size_map_min (KD_TREE ctor box_length, ikd_Tree.h:226) */
   int max_points;          /* capacity in points (valid + overflow chains); 0 -> 8M */
-  int max_blocks;          /* capacity in 4x4x4-voxel blocks; 0 -> max_points/4 */
+  int max_blocks;          /* capacity in 4x4x4-voxel blocks; 0 -> max_points/4.  Device memory ~1.5 KB per block, of
+                              which 76 B are the coarse level (one coarse cell per block at most: sparse content never
+                              fills it) */
   int device;              /* CUDA device ordinal */
 } flb_map_config;
 
