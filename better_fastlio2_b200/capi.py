@@ -77,6 +77,21 @@ class IcpConfig(C.Structure):
                 ("transformation_epsilon", C.c_double), ("euclidean_fitness_epsilon", C.c_double)]
 
 
+class FricpConfig(C.Structure):
+    _fields_ = [("mode", C.c_int), ("max_icp", C.c_int), ("stop", C.c_double), ("anderson_m", C.c_int),
+                ("nu_begin_k", C.c_double), ("nu_end_k", C.c_double), ("nu_alpha", C.c_double)]
+
+
+class FricpResult(C.Structure):
+    _fields_ = [("res_trans", C.c_double * 16), ("status", C.c_int), ("stages", C.c_int), ("iterations", C.c_int),
+                ("rejections", C.c_int), ("scale", C.c_double), ("mu_source", C.c_double * 3), ("mu_target", C.c_double * 3),
+                ("nu_begin", C.c_double), ("nu_end", C.c_double), ("energy", C.c_double), ("n_source", C.c_int),
+                ("n_target", C.c_int), ("n_source_finite", C.c_int), ("n_target_finite", C.c_int), ("log_n", C.c_int)]
+
+
+FRICP_STATUS = ["OK", "FEW_TARGET", "NO_SOURCE"]
+
+
 class IcpResult(C.Structure):
     _fields_ = [("final_transformation", C.c_float * 16), ("converged", C.c_int), ("iterations", C.c_int), ("state", C.c_int),
                 ("n_source", C.c_int), ("n_target", C.c_int), ("n_correspondences", C.c_int), ("fitness_score", C.c_double)]
@@ -106,6 +121,7 @@ EXPORTS = [
     "flb_keyframes_download", "flb_keyframes_info", "flb_keyframes_size", "flb_map_reconstruct_from_keyframes",
     "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
     "flb_keyframes_scan_context", "flb_keyframes_scan_contexts", "flb_keyframes_icp",
+    "flb_fricp_default_config", "flb_keyframes_fricp",
     "flb_frontend_camera_config", "flb_frontend_camera_image", "flb_frontend_points_colorize", "flb_frontend_points_to_imu",
 ]
 
@@ -205,6 +221,10 @@ def lib():
         L.flb_keyframes_scan_contexts.argtypes = [vp, vp, C.c_int, C.c_double, dp]
         L.flb_keyframes_icp.argtypes = [vp, vp, C.c_int, C.c_int, fp, fp, vp, C.c_int, C.c_int, fp, C.POINTER(IcpConfig),
                                         C.POINTER(IcpResult), vp, fp]
+        L.flb_fricp_default_config.argtypes = [C.POINTER(FricpConfig)]
+        L.flb_fricp_default_config.restype = None
+        L.flb_keyframes_fricp.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, fp, vp, C.c_int, fp, fp, C.POINTER(FricpConfig),
+                                          C.POINTER(FricpResult), vp, dp, dp, C.c_int]
         _lib = L
     return _lib
 
@@ -877,6 +897,51 @@ class KeyFrameStore:
         if correspondences:
             return res, idx[:r.n_source].copy(), d2[:r.n_source].copy()
         return res
+
+    def fricp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, mode=4, max_icp=100, stop=1e-5,
+              anderson_m=5, nu_begin_k=3.0, nu_end_k=1.0 / (3.0 * np.sqrt(3.0)), nu_alpha=0.5, correspondences=False, log=False,
+              log_cap=4096):
+        """The relocaliser's registration on the device (Registeration(mode).run(curCloud, nearCloud)): the host source
+        ((n,3) / (n,4) float32 x,y,z[,intensity], or (n,12) PointType records), moved by src_pose6 (initPose) when given,
+        onto the key frames tgt_ids each moved by tgt_pre_pose6 (pose_ext) when given and then by its tgt_poses6 row.
+        Returns a dict (res_trans (4,4) float64, status, status_name, stages, iterations, rejections, scale, mu_source,
+        mu_target, nu_begin, nu_end, energy, n_source, n_target, n_source_finite, n_target_finite) and, in this order when
+        asked for, the last pass's matched target index (-1: none) and residual of every source point, and the
+        per-iteration log ((k, 5): stage, energy, previous accepted energy, |T - T_prev|_F, accepted)."""
+        pts = np.ascontiguousarray(src_points, np.float32)
+        if pts.ndim != 2 or pts.shape[1] not in (3, 4, 12):
+            raise ValueError("src_points must be (n,3), (n,4) or (n,12) float32")
+        stride = 4 * pts.shape[1]
+        off_i = -1 if pts.shape[1] == 3 else (12 if pts.shape[1] == 4 else OFF_INTENSITY)
+        n = len(pts)
+        ids = np.ascontiguousarray(tgt_ids, np.int32).reshape(-1)
+        p6 = np.ascontiguousarray(tgt_poses6, np.float32).reshape(-1, 6)
+        if len(p6) != len(ids):
+            raise ValueError("one pose per target key frame")
+        pre = None if tgt_pre_pose6 is None else np.ascontiguousarray(tgt_pre_pose6, np.float32).reshape(6)
+        sp = None if src_pose6 is None else np.ascontiguousarray(src_pose6, np.float32).reshape(6)
+        cfg = FricpConfig(int(mode), int(max_icp), float(stop), int(anderson_m), float(nu_begin_k), float(nu_end_k), float(nu_alpha))
+        r = FricpResult()
+        idx = resid = lg = None
+        if correspondences:
+            idx = np.empty(max(n, 1), np.int32)
+            resid = np.empty(max(n, 1), np.float64)
+        if log:
+            lg = np.zeros((max(int(log_cap), 1), 5), np.float64)
+        _chk(lib().flb_keyframes_fricp(self.h, _p(pts) if n else None, n, stride, off_i, _p(sp), _p(ids) if len(ids) else None, len(ids),
+                                       _p(pre), _p(p6) if len(ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(resid), _p(lg),
+                                       int(log_cap) if log else 0))
+        res = {"res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
+               "status_name": FRICP_STATUS[r.status], "stages": r.stages, "iterations": r.iterations, "rejections": r.rejections,
+               "scale": r.scale, "mu_source": np.array(r.mu_source[:]), "mu_target": np.array(r.mu_target[:]),
+               "nu_begin": r.nu_begin, "nu_end": r.nu_end, "energy": r.energy, "n_source": r.n_source, "n_target": r.n_target,
+               "n_source_finite": r.n_source_finite, "n_target_finite": r.n_target_finite}
+        out = (res,)
+        if correspondences:
+            out += (idx[:n].copy(), resid[:n].copy())
+        if log:
+            out += (lg[:r.log_n].copy(),)
+        return out if len(out) > 1 else res
 
 
 def make_fov(cube_len=200.0, det_range=100.0):

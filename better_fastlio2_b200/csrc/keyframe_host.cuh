@@ -10,6 +10,9 @@
 struct IcpWork;                            // ICP scratch (icp_host.cuh)
 static void icp_release(IcpWork* w);
 static size_t icp_device_bytes(const IcpWork* w);
+struct FricpWork;                          // relocalisation registration scratch (fricp_host.cuh)
+static void fricp_release(FricpWork* w);
+static size_t fricp_device_bytes(const FricpWork* w);
 
 // ------------------------------------------------------------------------------------------------ map-side scratch
 // Kept with the map and only ever grown, like kf_raw / kf_in / kf_out: the readers run every kd_step key frames or on a
@@ -27,12 +30,14 @@ struct KfWork {
   DevBuf<unsigned> d_sc_keys;                  // Scan Context keys, SC_BINS per descriptor
   PinnedBuf<unsigned> h_sc_keys;               //   and their staging
   IcpWork* icp = nullptr;                      // flb_keyframes_icp's sub-maps, target index and reductions
+  FricpWork* fricp = nullptr;                  // flb_keyframes_fricp's clouds, target index, medians and reductions
 };
 
 static void kfw_release(KfWork* w) {
   if (!w) return;
   if (w->ev_seg) Q(cudaEventDestroy(w->ev_seg));
   icp_release(w->icp);
+  fricp_release(w->fricp);
   delete w;
 }
 
@@ -69,7 +74,8 @@ static int kf_scratch(flb_map* m, int n, bool curv, bool filter) {
 static long long kf_scratch_bytes(const flb_map* m) {
   size_t b = m->kf_raw.cap + m->kf_in.cap + m->kf_out.cap;   // device bytes (the pinned staging is not counted)
   if (const KfWork* w = m->kfw)
-    b += w->cin.cap + w->cout.cap + w->d_seg.cap + w->d_chunk.cap + w->d_sc_keys.cap + vg_device_bytes(w->vg) + icp_device_bytes(w->icp);
+    b += w->cin.cap + w->cout.cap + w->d_seg.cap + w->d_chunk.cap + w->d_sc_keys.cap + vg_device_bytes(w->vg) + icp_device_bytes(w->icp) +
+         fricp_device_bytes(w->fricp);
   return (long long)b;
 }
 

@@ -476,6 +476,57 @@ int flb_keyframes_icp(flb_keyframes* kf, const int* src_ids, int n_src, int src_
                       const float* src_pre_pose6, const int* tgt_ids, int n_tgt, int tgt_kind, const float* tgt_transforms,
                       const flb_icp_config* cfg, flb_icp_result* out, int* out_corr_index, float* out_corr_d2);
 
+/* ------------------------------------------------------------------------------------------------ relocalisation registration
+ * The online relocaliser's registration (pose_estimator::run, reg[0].run(curCloud, nearCloud), pose_estimator.cpp:180-269,
+ * :566-596): FRICP<3>::point_to_point as Registeration::run (include/FRICP-toolkit/registeration.h:36-175) calls it, for
+ * the four point-to-point modes.  Source = a host cloud (records of src_stride bytes, x, y, z floats first, intensity at
+ * src_off_intensity or < 0 for none), moved by transformPointCloud(.., pose6 src_pose6) when that is not NULL (initPose,
+ * :185).  Target = for every tgt_ids[j] the stored key frame moved by pose6 tgt_pre_pose6 (pose_ext; NULL: skipped) and
+ * then by pose6 tgt_poses6[j] (cloudKeyPoses6D), each stage rounding like transformPointCloud, concatenated in order
+ * (:189-194).  A point's index is its position in its cloud.  Non-finite points are dropped from both clouds; the clouds
+ * are scaled by max(|source extent|, |target extent|) and de-meaned in double; each iteration matches every source point
+ * to its exact nearest target point (double d², equal d²: the lower target index); Welsch weights, the weighted Kabsch
+ * step, Anderson acceleration on the SE(3) log and the ν schedule follow the reference.  DESIGN.md §9 states the contract
+ * and its deviations.  Every argument is checked before any device work; one synchronisation per iteration (two when
+ * Anderson rejects); the store and the map are not modified.  The clouds, the target index and the reduction buffers are
+ * map-side key-frame scratch (flb_keyframes_info, flb_map_release_keyframe_scratch). */
+#define FLB_FRICP_ICP 0                /* regMode 0: no robust function, no Anderson acceleration */
+#define FLB_FRICP_FAST 2               /* regMode 2: Anderson acceleration */
+#define FLB_FRICP_ROBUST 3             /* regMode 3: Welsch */
+#define FLB_FRICP_FAST_ROBUST 4        /* regMode 4: Welsch and Anderson acceleration (config/online_relo.yaml) */
+#define FLB_FRICP_OK 0                 /* registered */
+#define FLB_FRICP_FEW_TARGET 1         /* fewer than 2 finite target points: identity, nothing registered */
+#define FLB_FRICP_NO_SOURCE 2          /* no finite source point: identity, nothing registered */
+typedef struct flb_fricp_config {
+  int mode;                            /* FLB_FRICP_*: regMode 0, 2, 3 or 4; any other mode is rejected */
+  int max_icp;                         /* ICP::Parameters::max_icp (100): iterations per ν stage */
+  double stop;                         /* stop (1e-5): a stage ends when |T - T_prev|_F < stop (normalised units) */
+  int anderson_m;                      /* anderson_m (5), 1..5 */
+  double nu_begin_k, nu_end_k, nu_alpha; /* 3, 1/(3√3), 1/2 */
+} flb_fricp_config;
+typedef struct flb_fricp_result {
+  double res_trans[16];                /* Registeration::run's res_trans, row-major 4x4, translation in the caller's units */
+  int status;                          /* FLB_FRICP_OK / _FEW_TARGET / _NO_SOURCE */
+  int stages, iterations, rejections;  /* ν stages, ICP iterations over all stages, Anderson rejections */
+  double scale, mu_source[3], mu_target[3];   /* the normalisation: p_n = p / scale - mu */
+  double nu_begin, nu_end;             /* the Welsch scale's first and last value (0 without a robust function) */
+  double energy;                       /* convergence energy at the final ν */
+  int n_source, n_target;              /* source points; assembled target points */
+  int n_source_finite, n_target_finite;
+  int log_n;                           /* rows written to out_log */
+} flb_fricp_result;
+/* The reference's defaults (ICP::Parameters, ICP.h:518-566) with mode FLB_FRICP_FAST_ROBUST. */
+void flb_fricp_default_config(flb_fricp_config* cfg);
+/* Registers the source onto the target.  out_corr_index / out_resid (optional, n_src entries each) receive the last pass's
+ * matched target index and its residual |T x - q| in normalised units (-1 and +inf for a non-finite source point or when
+ * nothing was registered).  out_log (optional, log_cap rows of 5 doubles): per iteration the stage, the energy at the
+ * start of the iteration, the last accepted energy before it, |T - T_prev|_F and 1 (accepted or no Anderson) / 0
+ * (Anderson rejected). */
+int flb_keyframes_fricp(flb_keyframes* kf, const void* src_points, int n_src, int src_stride, int src_off_intensity,
+                        const float* src_pose6, const int* tgt_ids, int n_tgt, const float* tgt_pre_pose6, const float* tgt_poses6,
+                        const flb_fricp_config* cfg, flb_fricp_result* out, int* out_corr_index, double* out_resid,
+                        double* out_log, int log_cap);
+
 /* Stream access for callers that overlap work (returns a cudaStream_t as void*). */
 void* flb_session_stream(flb_session* s);
 int flb_session_sync(flb_session* s);

@@ -19,6 +19,9 @@
 //   // the ICP of performLoopClosure (:946-974) once the gate passed: the same selections, com = the SC yaw pose
 //   flb::IcpParams icp;  icp.setMaxCorrespondenceDistance(200); ...;  flb::IcpResult reg;
 //   keyframes.icp(curIds, curT, com, preIds, preT, icp, reg);  reg.hasConverged(), reg.getFitnessScore(), ...
+//   // the relocaliser (pose_estimator.cpp:184-198, :566-596), the prior session's key frames pushed back once:
+//   flb::FricpParams fr(regMode);  Eigen::MatrixXd T(4, 4);
+//   keyframes.fricp(*cloudBuffer[idx], initPose, nearIds, pose_ext, *poses6D, fr, T);
 //
 // Poses6D is anything with points[k].{x, y, z, roll, pitch, yaw} (pcl::PointCloud<PointTypePose>); an affine is
 // anything with operator()(row, col) (Eigen::Affine3f).  Clouds come back with x, y, z, intensity and curvature set
@@ -57,6 +60,16 @@ struct IcpResult {
   void getFinalTransformation(M& T) const {
     for (int i = 0; i < 4; ++i)
       for (int j = 0; j < 4; ++j) T(i, j) = r.final_transformation[4 * i + j];
+  }
+};
+
+// Registeration(regMode) of the relocaliser (registeration.h:24-33) with ICP::Parameters' values (ICP.h:518-566); the
+// mode numbers are the reference's: 0 ICP, 2 Fast ICP, 3 Robust ICP, 4 Fast and Robust ICP (config/online_relo.yaml).
+struct FricpParams {
+  flb_fricp_config cfg{};
+  explicit FricpParams(int regMode = FLB_FRICP_FAST_ROBUST) {
+    flb_fricp_default_config(&cfg);
+    cfg.mode = regMode;
   }
 };
 
@@ -177,6 +190,32 @@ class KeyFrameStore {
     return ok(flb_keyframes_icp(kf_, curIds.data(), (int)curIds.size(), FLB_KF_AFFINE, a.data(), pre, preIds.data(), (int)preIds.size(),
                                 FLB_KF_AFFINE, b.data(), &params.cfg, &result.r, nullptr, nullptr),
               "icp");
+  }
+
+  // pose_estimator::run's registration (pose_estimator.cpp:184-198) with the prior session's key frames in the store:
+  // curCloud moved by initPose, onto the key frames ids each moved by pose_ext and then by poses6D.points[ids[j]], with
+  // Registeration(params.cfg.mode).run.  T receives res_trans (anything with operator()(row, col) of a 4x4, i.e. the
+  // Eigen::MatrixXd the node reads at :197-198, sized by the caller).  Pose is anything with x, y, z, roll, pitch, yaw
+  // (PointTypePose); info (optional) receives the whole result.
+  template <class Cloud, class Pose, class Poses6D, class Mat>
+  bool fricp(const Cloud& curCloud, const Pose& initPose, const std::vector<int>& ids, const Pose& pose_ext, const Poses6D& poses6D,
+             const FricpParams& params, Mat& T, flb_fricp_result* info = nullptr) {
+    typedef typename std::remove_reference<decltype(curCloud.points[0])>::type P;
+    const int n = (int)curCloud.points.size();
+    const P* p0 = n ? &curCloud.points[0] : nullptr;
+    const int off_i = n ? (int)((const char*)&p0->intensity - (const char*)p0) : -1;
+    const float init6[6] = {initPose.x, initPose.y, initPose.z, initPose.roll, initPose.pitch, initPose.yaw};
+    const float ext6[6] = {pose_ext.x, pose_ext.y, pose_ext.z, pose_ext.roll, pose_ext.pitch, pose_ext.yaw};
+    const std::vector<float> p6 = poses6(ids, poses6D);
+    flb_fricp_result r{};
+    if (!ok(flb_keyframes_fricp(kf_, p0, n, (int)sizeof(P), off_i, init6, ids.data(), (int)ids.size(), ext6, p6.data(), &params.cfg, &r,
+                                nullptr, nullptr, nullptr, 0),
+            "fricp"))
+      return false;
+    for (int i = 0; i < 4; ++i)
+      for (int j = 0; j < 4; ++j) T(i, j) = r.res_trans[4 * i + j];
+    if (info) *info = r;
+    return true;
   }
 
   // pcl::copyPointCloud(*surfCloudKeyFrames[k], out)
