@@ -2,73 +2,31 @@
 // nearCloud) with Registeration(regMode), include/FRICP-toolkit/registeration.h:36-175) for regMode 0, 2, 3 and 4: a host
 // source cloud onto a target assembled from the device key-frame store with two transform stages per key frame
 // (transformPointCloud(transformPointCloud(cloud, &pose_ext), &poses6D[k]), pose_estimator.cpp:189-194).  The clouds are
-// normalised on the device (extent, fixed-order double means), the loop ICP's index is built once over the target, the
-// Welsch scale's end value comes from an exact 7-NN self-query and a device sort, and every iteration is one double 1-NN
-// pass, one fused reduction (energy and weighted moments), one small copy and one synchronisation.  The 3x3 SVD, the
-// SE(3) log / exp, Anderson acceleration and the stopping tests run here on the host.  DESIGN.md §9 states the contract.
-// Included after icp_host.cuh.
+// normalised on the device (extent, fixed-order double means), the loop ICP's index (icp_host.cuh) is built once over
+// the target, the Welsch scale's end value comes from an exact 7-NN self-query and a device sort, and every iteration is
+// one double 1-NN pass, one fused reduction (energy and weighted moments), one small copy and one synchronisation.  The
+// 3x3 SVD, the SE(3) log / exp, Anderson acceleration and the stopping tests run here on the host.  DESIGN.md §9 states
+// the contract.  Included after icp_host.cuh.
 #pragma once
 #include <cfloat>
 #include <cmath>
 
 #include "fricp_kernels.cuh"
 
-// Grow-only scratch, held by the map's KfWork (counted in map_scratch_bytes, freed with the rest of it).
-struct FricpWork {
-  DevBuf<unsigned char> raw;                     // staged source records
-  DevBuf<float4> src_raw, src, tgt_a, tgt, tgtf;  // uploaded / pre-transformed source, the two target stages, float target
-  DevBuf<double4> x, tn, sorted_d;               // normalised source, normalised target, sorted finite target (w = index)
-  DevBuf<float4> sorted;                         // its float rounding (the coarse boxes)
-  DevBuf<unsigned> keys_a, keys_b;
-  DevBuf<int> vals_a, vals_b, order, pos, open;
-  DevBuf<double> d2, med, sort_a, sort_b;        // 1-NN d²; 7-NN medians; sort input / output of a median
-  DevBuf<int> cs, corr;
-  DevBuf<IcpBox> box;
-  DevBuf<unsigned char> tmp;                     // CUB temporary storage
-  DevBuf<double> partials, sums;                 // reduction block partials; reduction records
-  DevBuf<unsigned> misc;                         // bounds (7 words per cloud), open count, reduction counter
-  PinnedBuf<unsigned> h_misc;
-  PinnedBuf<double> h_sums;
-};
-
-static void fricp_release(FricpWork* w) { delete w; }
-
-static size_t fricp_device_bytes(const FricpWork* w) {
-  if (!w) return 0;
-  return w->raw.cap + w->src_raw.cap + w->src.cap + w->tgt_a.cap + w->tgt.cap + w->tgtf.cap + w->x.cap + w->tn.cap + w->sorted_d.cap +
-         w->sorted.cap + w->keys_a.cap + w->keys_b.cap + w->vals_a.cap + w->vals_b.cap + w->order.cap + w->pos.cap + w->open.cap +
-         w->d2.cap + w->med.cap + w->sort_a.cap + w->sort_b.cap + w->cs.cap + w->corr.cap + w->box.cap + w->tmp.cap + w->partials.cap +
-         w->sums.cap + w->misc.cap;
-}
-
-constexpr int FR_MISC_SRC = 0, FR_MISC_TGT = 8, FR_MISC_GRID = 16, FR_MISC_OPEN = 24, FR_MISC_COUNTER = 25, FR_MISC_WORDS = 32;
 constexpr int FR_SUM_MEAN_S = 0, FR_SUM_MEAN_T = 4, FR_SUM_STEP = 8, FR_SUM_MED = 32, FR_SUM_WORDS = 40;
 
-static int fricp_scratch(flb_map* m, FricpWork*& wp, int n_s, int n_t, bool pre_src, bool two_stage) {
-  if (kf_work(m)) return 1;
-  KfWork& k = *m->kfw;
-  if (!k.fricp) {
-    k.fricp = new (std::nothrow) FricpWork();
-    if (!k.fricp) return set_err("out of host memory");
-  }
-  wp = k.fricp;
-  FricpWork& w = *wp;
+static int fricp_scratch(flb_map* m, KfWork& k, int n_s, int n_t, bool pre_src, bool two_stage) {
+  FricpWork& w = k.fricp;
   const size_t ps = sizeof(float4) * (size_t)n_s, pt = sizeof(float4) * (size_t)n_t;
   const int nk = std::max(n_s, n_t);
-  size_t t1 = 0, t2 = 0;
-  CU(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, nk));
+  size_t t2 = 0;
   CU(cub::DeviceRadixSort::SortKeys(nullptr, t2, (const double*)nullptr, (double*)nullptr, nk));
-  const int red_blocks = m->sm_count * 2;
-  if (kf_grow(w.src_raw, ps) || (pre_src && kf_grow(w.src, ps)) || (two_stage && kf_grow(w.tgt_a, pt)) || kf_grow(w.tgt, pt) ||
-      kf_grow(w.tgtf, pt) || kf_grow(w.x, sizeof(double4) * (size_t)n_s) || kf_grow(w.tn, sizeof(double4) * (size_t)n_t) ||
-      kf_grow(w.sorted_d, sizeof(double4) * (size_t)n_t) || kf_grow(w.sorted, pt) || kf_grow(w.keys_a, sizeof(unsigned) * (size_t)nk) ||
-      kf_grow(w.keys_b, sizeof(unsigned) * (size_t)nk) || kf_grow(w.vals_a, sizeof(int) * (size_t)nk) ||
-      kf_grow(w.vals_b, sizeof(int) * (size_t)nk) || kf_grow(w.order, sizeof(int) * (size_t)n_s) || kf_grow(w.pos, sizeof(int) * (size_t)n_s) ||
-      kf_grow(w.open, sizeof(int) * (size_t)nk) || kf_grow(w.d2, sizeof(double) * (size_t)n_s) || kf_grow(w.med, sizeof(double) * (size_t)n_t) ||
+  if (icp_index_scratch(m, k.index, n_s, n_t, t2) || kf_grow(w.src_raw, ps) || (pre_src && kf_grow(w.src, ps)) ||
+      (two_stage && kf_grow(w.tgt_a, pt)) || kf_grow(w.tgt, pt) || kf_grow(w.tgtf, pt) || kf_grow(w.x, sizeof(double4) * (size_t)n_s) ||
+      kf_grow(w.tn, sizeof(double4) * (size_t)n_t) || kf_grow(w.sorted_d, sizeof(double4) * (size_t)n_t) ||
+      kf_grow(w.pos, sizeof(int) * (size_t)n_s) || kf_grow(w.d2, sizeof(double) * (size_t)n_s) || kf_grow(w.med, sizeof(double) * (size_t)n_t) ||
       kf_grow(w.sort_a, sizeof(double) * (size_t)nk) || kf_grow(w.sort_b, sizeof(double) * (size_t)nk) ||
-      kf_grow(w.corr, sizeof(int) * (size_t)n_s) || kf_grow(w.tmp, std::max(t1, t2) + 256) ||
-      grow(w.partials, sizeof(double) * FR_RED * (size_t)red_blocks, 0) || grow(w.sums, sizeof(double) * FR_SUM_WORDS, 0) ||
-      grow(w.misc, sizeof(unsigned) * FR_MISC_WORDS, 0) || grow(w.h_misc, sizeof(unsigned) * FR_MISC_WORDS, 0) ||
+      kf_grow(w.corr, sizeof(int) * (size_t)n_s) || grow(w.sums, sizeof(double) * FR_SUM_WORDS, 0) ||
       grow(w.h_sums, sizeof(double) * FR_SUM_WORDS, 0))
     return 1;
   return 0;
@@ -266,50 +224,33 @@ static void fr_kabsch(const double* S, double* T) {
 }
 
 // ------------------------------------------------------------------------------------------------ device passes
-struct FrCall {
-  flb_map* m;
-  FricpWork* w;
-  IcpGrid g;
-  IcpBox* box;
-  int n_s, n_fin_t;
-};
-
-static int fr_red_blocks(const flb_map* m) { return m->sm_count * 2; }
-
-template <int K, class Op>
-static int fr_reduce(flb_map* m, FricpWork& w, int n, const Op& op, double* out) {
-  k_fr_reduce<K, Op><<<fr_red_blocks(m), 256, 0, m->stream>>>(n, op, w.partials.p, w.misc.p + FR_MISC_COUNTER, out);
-  m->launches++;
-  CU(cudaGetLastError());
-  return 0;
-}
-
 // One 1-NN pass with T applied in the pass, then the step record (energy and weighted moments at nu) and its copy.  The
 // caller synchronises.
-static int fr_pass(const FrCall& c, const double* T, bool nn, double nu, bool welsch) {
-  flb_map* m = c.m;
-  FricpWork& w = *c.w;
+static int fr_pass(flb_map* m, KfWork& k, const IcpGrid& g, int n_s, const double* T, bool nn, double nu, bool welsch) {
+  IcpIndex& x = k.index;
+  FricpWork& w = k.fricp;
   if (nn) {
     FrXf xf;
     memcpy(xf.m, T, sizeof(xf.m));
-    int* open_n = (int*)(w.misc.p + FR_MISC_OPEN);
+    int* open_n = (int*)(x.misc.p + ICP_MISC_OPEN);
     CU(cudaMemsetAsync(open_n, 0, sizeof(int), m->stream));
-    k_fr_nn<<<grid_for(c.n_s, 256, m->sm_count * 8), 256, 0, m->stream>>>(c.g, xf, w.order.p, c.n_s, w.x.p, w.sorted_d.p, w.cs.p, w.pos.p,
-                                                                          w.d2.p, w.open.p, open_n);
-    k_fr_nn_far<<<m->sm_count * 8, 256, 0, m->stream>>>(c.g, xf, w.open.p, open_n, w.x.p, w.sorted_d.p, w.cs.p, c.box, w.pos.p, w.d2.p);
+    k_fr_nn<<<grid_for(n_s, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, xf, x.order.p, n_s, w.x.p, w.sorted_d.p, x.cs.p, w.pos.p,
+                                                                        w.d2.p, x.open.p, open_n);
+    k_fr_nn_far<<<m->sm_count * 8, 256, 0, m->stream>>>(g, xf, x.open.p, open_n, w.x.p, w.sorted_d.p, x.cs.p, x.box.p, w.pos.p, w.d2.p);
     m->launches += 2;
     CU(cudaGetLastError());
   }
   const FrStepOp op{w.x.p, w.sorted_d.p, w.pos.p, w.d2.p, nu, welsch ? 1 : 0};
-  if (fr_reduce<FR_RED>(m, w, c.n_s, op, w.sums.p + FR_SUM_STEP)) return 1;
+  if (icp_reduce<FR_RED>(m, x, n_s, op, w.sums.p + FR_SUM_STEP)) return 1;
   CU(cudaMemcpyAsync(w.h_sums.p + FR_SUM_STEP, w.sums.p + FR_SUM_STEP, sizeof(double) * FR_RED, cudaMemcpyDeviceToHost, m->stream));
   return 0;
 }
 
 // igl::median of the first n values of `in` (non-finite ones sort last): a device radix sort, then the middle one or two.
-static int fr_median(flb_map* m, FricpWork& w, const double* in, int n_all, int n, double* out) {
-  size_t tb = w.tmp.cap;
-  CU(cub::DeviceRadixSort::SortKeys(w.tmp.p, tb, in, w.sort_b.p, n_all, 0, 64, m->stream));
+static int fr_median(flb_map* m, KfWork& k, const double* in, int n_all, int n, double* out) {
+  FricpWork& w = k.fricp;
+  size_t tb = k.index.tmp.cap;
+  CU(cub::DeviceRadixSort::SortKeys(k.index.tmp.p, tb, in, w.sort_b.p, n_all, 0, 64, m->stream));
   m->launches += 5;   // the radix sort's kernels
   const int h = n / 2;
   const int first = n % 2 == 0 ? h - 1 : h, cnt = n % 2 == 0 ? 2 : 1;
@@ -387,9 +328,10 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
   }
   flb_map* m = k->map;
   CU(cudaSetDevice(m->cfg.device));
-  FricpWork* wp = nullptr;
-  if (fricp_scratch(m, wp, n_s, n_t, src_pose6 != nullptr, tgt_pre_pose6 != nullptr)) return 1;
-  FricpWork& w = *wp;
+  if (kf_work(m) || fricp_scratch(m, *m->kfw, n_s, n_t, src_pose6 != nullptr, tgt_pre_pose6 != nullptr)) return 1;
+  KfWork& kw = *m->kfw;
+  IcpIndex& x = kw.index;
+  FricpWork& w = kw.fricp;
 
   // curCloud = transformPointCloud(cloud, &initPose) (pose_estimator.cpp:185)
   if (upload_records(m, m->stream, w.raw, 0, src_pts, n_s, src_stride, src_off_intensity, -1, w.src_raw.p, nullptr)) return 1;
@@ -419,18 +361,9 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
   }
 
   // finite counts and boxes of both clouds -> scale (registeration.h:47-53)
-  unsigned init[FR_MISC_WORDS] = {};
-  for (int b : {FR_MISC_SRC, FR_MISC_TGT, FR_MISC_GRID})
-    for (int a = 0; a < 3; ++a) init[b + a] = ~0u;
-  memcpy(w.h_misc.p, init, sizeof(init));
-  CU(cudaMemcpyAsync(w.misc.p, w.h_misc.p, sizeof(init), cudaMemcpyHostToDevice, m->stream));
-  k_icp_bounds<<<grid_for(n_s, 256, m->sm_count * 4), 256, 0, m->stream>>>(src, n_s, w.misc.p + FR_MISC_SRC);
-  k_icp_bounds<<<grid_for(n_t, 256, m->sm_count * 4), 256, 0, m->stream>>>(w.tgt.p, n_t, w.misc.p + FR_MISC_TGT);
-  m->launches += 2;
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(w.h_misc.p, w.misc.p, sizeof(unsigned) * 16, cudaMemcpyDeviceToHost, m->stream));
-  CU(cudaStreamSynchronize(m->stream));
-  const int n_fs = (int)w.h_misc.p[FR_MISC_SRC + 6], n_ft = (int)w.h_misc.p[FR_MISC_TGT + 6];
+  float lo[2][3], hi[2][3];
+  int n_fs = 0, n_ft = 0;
+  if (icp_bounds(m, x, src, n_s, lo[0], hi[0], &n_fs) || icp_bounds(m, x, w.tgt.p, n_t, lo[1], hi[1], &n_ft)) return 1;
   res.n_source_finite = n_fs;
   res.n_target_finite = n_ft;
   if (n_ft < 2 || n_fs == 0) {
@@ -440,17 +373,16 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
   }
   double ext[2];
   for (int c = 0; c < 2; ++c) {
-    const unsigned* b = w.h_misc.p + (c ? FR_MISC_TGT : FR_MISC_SRC);
     double e[3];
-    for (int a = 0; a < 3; ++a) e[a] = (double)icp_fkey(b[3 + a]) - (double)icp_fkey(b[a]);
+    for (int a = 0; a < 3; ++a) e[a] = (double)hi[c][a] - (double)lo[c][a];
     ext[c] = std::sqrt((e[0] * e[0] + e[1] * e[1]) + e[2] * e[2]);
   }
   double scale = std::max(ext[0], ext[1]);
   if (!(scale > 0)) scale = 1.0;   // every finite point of both clouds at one place: nothing to scale
 
   // means (fixed order), normalised clouds, the float target for the index
-  if (fr_reduce<3>(m, w, n_s, FrMeanOp{src, scale}, w.sums.p + FR_SUM_MEAN_S) ||
-      fr_reduce<3>(m, w, n_t, FrMeanOp{w.tgt.p, scale}, w.sums.p + FR_SUM_MEAN_T))
+  if (icp_reduce<3>(m, x, n_s, FrMeanOp{src, scale}, w.sums.p + FR_SUM_MEAN_S) ||
+      icp_reduce<3>(m, x, n_t, FrMeanOp{w.tgt.p, scale}, w.sums.p + FR_SUM_MEAN_T))
     return 1;
   CU(cudaMemcpyAsync(w.h_sums.p, w.sums.p, sizeof(double) * 8, cudaMemcpyDeviceToHost, m->stream));
   CU(cudaStreamSynchronize(m->stream));
@@ -464,37 +396,21 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
   CU(cudaMemcpyAsync(w.sums.p, w.h_sums.p, sizeof(double) * 8, cudaMemcpyHostToDevice, m->stream));
   k_fr_normalise<<<grid_for(n_s, 256, m->sm_count * 8), 256, 0, m->stream>>>(src, n_s, scale, w.sums.p + FR_SUM_MEAN_S, w.x.p, nullptr);
   k_fr_normalise<<<grid_for(n_t, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.tgt.p, n_t, scale, w.sums.p + FR_SUM_MEAN_T, w.tn.p, w.tgtf.p);
-  k_icp_bounds<<<grid_for(n_t, 256, m->sm_count * 4), 256, 0, m->stream>>>(w.tgtf.p, n_t, w.misc.p + FR_MISC_GRID);
-  m->launches += 3;
+  m->launches += 2;
   CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(w.h_misc.p + FR_MISC_GRID, w.misc.p + FR_MISC_GRID, sizeof(unsigned) * 7, cudaMemcpyDeviceToHost, m->stream));
-  CU(cudaStreamSynchronize(m->stream));
   res.scale = scale;
   for (int a = 0; a < 3; ++a) { res.mu_source[a] = mu_s[a]; res.mu_target[a] = mu_t[a]; }
 
-  // the loop ICP's index over the float normalised target, the sorted double target, the source's visiting order
-  float lo[3], hi[3];
-  for (int a = 0; a < 3; ++a) { lo[a] = icp_fkey(w.h_misc.p[FR_MISC_GRID + a]); hi[a] = icp_fkey(w.h_misc.p[FR_MISC_GRID + 3 + a]); }
-  const IcpGrid g = icp_grid(lo, hi, n_ft);
-  const unsigned n_cells = (unsigned)g.gx * g.gy * g.gz;
-  const int n_coarse = g.cx * g.cy * g.cz;
-  if (grow(w.cs, sizeof(int) * ((size_t)n_cells + 1), 0) || grow(w.box, sizeof(IcpBox) * (size_t)n_coarse, 0)) return 1;
-  const int gt = grid_for(n_t, 256, m->sm_count * 8), gs = grid_for(n_s, 256, m->sm_count * 8);
-  size_t tb = w.tmp.cap;
-  k_icp_keys<<<gt, 256, 0, m->stream>>>(g, w.tgtf.p, n_t, w.keys_a.p, w.vals_a.p);
-  CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)w.keys_a.p, w.keys_b.p, (const int*)w.vals_a.p, w.vals_b.p, n_t, 0, 32,
-                                     m->stream));
-  k_icp_gather<<<grid_for(n_ft, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.vals_b.p, w.tgtf.p, n_ft, w.sorted.p);
-  k_fr_gather<<<grid_for(n_ft, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.vals_b.p, w.tn.p, n_ft, w.sorted_d.p);
-  k_icp_cell_start<<<grid_for(n_ft + 1, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.keys_b.p, n_ft, n_cells, w.cs.p);
-  k_icp_coarse_boxes<<<grid_for(n_coarse, 8, m->sm_count * 8), 256, 0, m->stream>>>(w.sorted.p, w.cs.p, n_coarse, w.box.p);
-  k_fr_keys<<<gs, 256, 0, m->stream>>>(g, w.x.p, n_s, w.keys_a.p, w.vals_a.p);
-  tb = w.tmp.cap;
-  CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)w.keys_a.p, w.keys_b.p, (const int*)w.vals_a.p, w.order.p, n_s, 0, 32,
-                                     m->stream));
-  m->launches += 7 + 2 * 5;   // + the radix sorts' kernels
-  CU(cudaGetLastError());
-  const FrCall call{m, wp, g, w.box.p, n_s, n_ft};
+  // the loop ICP's index over the float normalised target (its finite points are the target's), the sorted double
+  // target beside it, the source's visiting order
+  IcpGrid g{};
+  int n_fin = 0;
+  if (icp_index(m, x, w.tgtf.p, n_t, &g, &n_fin)) return 1;
+  const int gs = grid_for(n_s, 256, m->sm_count * 8);
+  k_fr_gather<<<grid_for(n_ft, 256, m->sm_count * 8), 256, 0, m->stream>>>(x.vals_b.p, w.tn.p, n_ft, w.sorted_d.p);
+  k_fr_keys<<<gs, 256, 0, m->stream>>>(g, w.x.p, n_s, x.keys_a.p, x.vals_a.p);
+  m->launches += 2;
+  if (icp_order(m, x, n_s)) return 1;
 
   // FRICP<3>::point_to_point (FRICP.h:382-543)
   const int mode = cfg->mode;
@@ -505,24 +421,24 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
   memcpy(To2, T, sizeof(T));
   double nu1 = 1, nu2 = 1;
   if (welsch) {   // :421-436: nu_end from the target's 7-NN median spacing, nu_begin from the initial residuals' median
-    if (fr_pass(call, T, true, 1.0, false)) return 1;
-    int* open_n = (int*)(w.misc.p + FR_MISC_OPEN);
+    if (fr_pass(m, kw, g, n_s, T, true, 1.0, false)) return 1;
+    int* open_n = (int*)(x.misc.p + ICP_MISC_OPEN);
     CU(cudaMemsetAsync(open_n, 0, sizeof(int), m->stream));
     const int kk = std::min(7, n_ft);
-    k_fr_knn7<<<grid_for(n_ft, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, n_ft, kk, w.sorted_d.p, w.cs.p, w.med.p, w.open.p, open_n);
-    k_fr_knn7_far<<<grid_for(n_ft, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, kk, w.open.p, open_n, w.sorted_d.p, w.cs.p, w.box.p, w.med.p);
+    k_fr_knn7<<<grid_for(n_ft, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, n_ft, kk, w.sorted_d.p, x.cs.p, w.med.p, x.open.p, open_n);
+    k_fr_knn7_far<<<grid_for(n_ft, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, kk, x.open.p, open_n, w.sorted_d.p, x.cs.p, x.box.p, w.med.p);
     k_fr_resid<<<gs, 256, 0, m->stream>>>(w.d2.p, n_s, w.sort_a.p);
     m->launches += 3;
     CU(cudaGetLastError());
     double med_t = 0, med_r = 0;
-    if (fr_median(m, w, w.med.p, n_ft, n_ft, &med_t) || fr_median(m, w, w.sort_a.p, n_s, n_fs, &med_r)) return 1;
+    if (fr_median(m, kw, w.med.p, n_ft, n_ft, &med_t) || fr_median(m, kw, w.sort_a.p, n_s, n_fs, &med_r)) return 1;
     nu2 = cfg->nu_end_k * std::sqrt(med_t);
     nu1 = std::max(cfg->nu_begin_k * med_r, nu2);
     res.nu_begin = nu1;
     res.nu_end = nu2;
-    if (fr_pass(call, T, false, nu1, true)) return 1;
+    if (fr_pass(m, kw, g, n_s, T, false, nu1, true)) return 1;
   } else {
-    if (fr_pass(call, T, true, nu1, false)) return 1;
+    if (fr_pass(m, kw, g, n_s, T, true, nu1, false)) return 1;
   }
   CU(cudaStreamSynchronize(m->stream));
   double S[FR_RED];
@@ -547,7 +463,7 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
           ++res.rejections;
           fr_log(SVD_T, L);
           aa.replace(L);
-          if (fr_pass(call, SVD_T, true, nu1, welsch)) return 1;
+          if (fr_pass(m, kw, g, n_s, SVD_T, true, nu1, welsch)) return 1;
           CU(cudaStreamSynchronize(m->stream));
           memcpy(S, w.h_sums.p + FR_SUM_STEP, sizeof(S));
           last_energy = S[16];
@@ -561,7 +477,7 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
         fr_log(T, L);
         fr_exp(aa.compute(L), T);
       }
-      if (fr_pass(call, T, true, nu1, welsch)) return 1;
+      if (fr_pass(m, kw, g, n_s, T, true, nu1, welsch)) return 1;
       CU(cudaStreamSynchronize(m->stream));
       memcpy(S, w.h_sums.p + FR_SUM_STEP, sizeof(S));
       double s2 = 0;
@@ -585,7 +501,7 @@ extern "C" int flb_keyframes_fricp(flb_keyframes* k, const void* src_pts, int n_
         aa.reset(L);
         last_energy = DBL_MAX;
       }
-      if (fr_pass(call, T, false, nu1, true)) return 1;   // the energies and weights at the new scale
+      if (fr_pass(m, kw, g, n_s, T, false, nu1, true)) return 1;   // the energies and weights at the new scale
       CU(cudaStreamSynchronize(m->stream));
       memcpy(S, w.h_sums.p + FR_SUM_STEP, sizeof(S));
     }

@@ -1,72 +1,33 @@
 // icp_host.cuh — performLoopClosure's ICP (laserMapping.cpp:946-974, pcl::IterativeClosestPoint 1.10 with the settings of
-// :947-952 and an identity guess) between two selections of the device key-frame store.  Both sub-maps are assembled by
-// k_kf_assemble into map-side scratch exactly as flb_keyframes_assemble writes them; the source's pre-transform
-// (transformPointCloud(cureKeyframeCloud, &com), :954-962) is one more k_kf_assemble segment over the assembled source.
-// The target index is built once per call; each iteration is one exact 1-NN pass and two fixed-order double reductions
-// on the map stream, one small copy and one synchronisation.  The 3x3 SVD, the 4x4 compositions and the convergence test
-// run here on the host between iterations.  The contract is written out in DESIGN.md §9.  Included after
-// scan_context_host.cuh.
+// :947-952 and an identity guess) between two selections of the device key-frame store, and the host side of the grid
+// index both registrations use (icp_bounds, icp_index, icp_order, icp_reduce over KfWork's IcpIndex).  Both sub-maps are
+// assembled by k_kf_assemble into map-side scratch exactly as flb_keyframes_assemble writes them; the source's
+// pre-transform (transformPointCloud(cureKeyframeCloud, &com), :954-962) is one more k_kf_assemble segment over the
+// assembled source.  The target index is built once per call; each iteration is one exact 1-NN pass and two fixed-order
+// double reductions on the map stream, one small copy and one synchronisation.  The 3x3 SVD, the 4x4 compositions and the
+// convergence test run here on the host between iterations.  The contract is written out in DESIGN.md §9.  Included
+// after scan_context_host.cuh.
 #pragma once
 #include <cfloat>
 #include <cmath>
 
 #include "icp_kernels.cuh"
 
-// Grow-only ICP scratch, held by the map's KfWork (counted in map_scratch_bytes, freed with the rest of it).
-struct IcpWork {
-  DevBuf<float4> src_raw, src, x, tgt, sorted;   // assembled source, pre-transformed source, input_transformed, target,
-                                                 // sorted finite target (w = original index)
-  DevBuf<unsigned> keys_a, keys_b;               // radix-sort keys
-  DevBuf<int> vals_a, vals_b, order;             // radix-sort values; source visiting order
-  DevBuf<int> corr, open;                        // nearest target per source; open queries of the thread path
-  DevBuf<float> corr_d2;
-  DevBuf<int> cs;                                // CSR cell offsets (n_cells + 1)
-  DevBuf<IcpBox> box;                            // coarse-cell point boxes
-  DevBuf<unsigned char> tmp;                     // CUB temporary storage
-  DevBuf<double> partials;                       // reduction block partials
-  DevBuf<unsigned> misc;                         // bounds keys (6), finite count, open count, reduction counter
-  DevBuf<IcpSums> sums;
-  PinnedBuf<unsigned> h_misc;
-  PinnedBuf<IcpSums> h_sums;
-};
-
-static void icp_release(IcpWork* w) { delete w; }
-
-static size_t icp_device_bytes(const IcpWork* w) {
-  if (!w) return 0;
-  return w->src_raw.cap + w->src.cap + w->x.cap + w->tgt.cap + w->sorted.cap + w->keys_a.cap + w->keys_b.cap + w->vals_a.cap +
-         w->vals_b.cap + w->order.cap + w->corr.cap + w->open.cap + w->corr_d2.cap + w->cs.cap + w->box.cap + w->tmp.cap +
-         w->partials.cap + w->misc.cap + w->sums.cap;
-}
-
-constexpr int ICP_MISC_OPEN = 7, ICP_MISC_COUNTER = 8, ICP_MISC_WORDS = 16;
+constexpr int ICP_MISC_OPEN = 7, ICP_MISC_COUNTER = 8, ICP_MISC_WORDS = 9;   // after the bounds words of k_icp_bounds
 constexpr double ICP_CELLS_PER_POINT = 8.0;     // dense fine cells over the target box per finite target point
 constexpr double ICP_MAX_CELLS = 134217728.0;   // 2^27 fine cells (512 MB of offsets) at most
 
-static int icp_work(flb_map* m, IcpWork** out) {
-  if (kf_work(m)) return 1;
-  KfWork& k = *m->kfw;
-  if (!k.icp) {
-    k.icp = new (std::nothrow) IcpWork();
-    if (!k.icp) return set_err("out of host memory");
-  }
-  *out = k.icp;
-  return 0;
-}
-
-// Scratch that follows the sizes of the two selections (the grid's buffers are grown once the grid is known).
-static int icp_scratch(flb_map* m, IcpWork& w, int n_s, int n_t, bool pre) {
-  const size_t ps = sizeof(float4) * (size_t)n_s, pt = sizeof(float4) * (size_t)n_t, is = sizeof(int) * (size_t)n_s;
+// The index's scratch for n_s queries and a target of n_t points (the grid's buffers are grown once the grid is known);
+// tmp_bytes: the caller's own CUB temporary storage beside the index's radix sorts.
+static int icp_index_scratch(flb_map* m, IcpIndex& x, int n_s, int n_t, size_t tmp_bytes) {
   const int nk = std::max(n_s, n_t);
   const size_t ik = sizeof(int) * (size_t)nk;
   size_t t1 = 0;
   CU(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const unsigned*)nullptr, (unsigned*)nullptr, (const int*)nullptr, (int*)nullptr, nk));
-  const int red_blocks = m->sm_count * 2;
-  if (kf_grow(w.src_raw, ps) || (pre && kf_grow(w.src, ps)) || kf_grow(w.x, ps) || kf_grow(w.tgt, pt) || kf_grow(w.sorted, pt) ||
-      kf_grow(w.keys_a, ik) || kf_grow(w.keys_b, ik) || kf_grow(w.vals_a, ik) || kf_grow(w.vals_b, ik) || kf_grow(w.order, is) ||
-      kf_grow(w.corr, is) || kf_grow(w.open, is) || kf_grow(w.corr_d2, sizeof(float) * (size_t)n_s) || kf_grow(w.tmp, t1 + 256) ||
-      grow(w.partials, sizeof(double) * ICP_RED * (size_t)red_blocks, 0) || grow(w.misc, sizeof(unsigned) * ICP_MISC_WORDS, 0) ||
-      grow(w.h_misc, sizeof(unsigned) * ICP_MISC_WORDS, 0) || grow(w.sums, sizeof(IcpSums), 0) || grow(w.h_sums, sizeof(IcpSums), 0))
+  if (kf_grow(x.sorted, sizeof(float4) * (size_t)n_t) || kf_grow(x.keys_a, ik) || kf_grow(x.keys_b, ik) || kf_grow(x.vals_a, ik) ||
+      kf_grow(x.vals_b, ik) || kf_grow(x.order, sizeof(int) * (size_t)n_s) || kf_grow(x.open, ik) ||
+      kf_grow(x.tmp, std::max(t1, tmp_bytes) + 256) || grow(x.partials, sizeof(double) * ICP_RED_MAX * (size_t)m->sm_count * 2, 0) ||
+      grow(x.misc, sizeof(unsigned) * ICP_MISC_WORDS, 0) || grow(x.h_misc, sizeof(unsigned) * ICP_MISC_WORDS, 0))
     return 1;
   return 0;
 }
@@ -114,6 +75,64 @@ static IcpGrid icp_grid(const float* lo, const float* hi, int n_fin) {
   g.slack = 1e-3f * g.e + 4e-6f * (float)(amax + L);
   g.cx = g.gx / ICP_C; g.cy = g.gy / ICP_C; g.cz = g.gz / ICP_C;
   return g;
+}
+
+// The finite count and box of p[0, n) (k_icp_bounds, read back); resets the open count and the reduction counter too.
+static int icp_bounds(flb_map* m, IcpIndex& x, const float4* p, int n, float* lo, float* hi, int* n_fin) {
+  const unsigned init[ICP_MISC_WORDS] = {~0u, ~0u, ~0u};
+  memcpy(x.h_misc.p, init, sizeof(init));
+  CU(cudaMemcpyAsync(x.misc.p, x.h_misc.p, sizeof(init), cudaMemcpyHostToDevice, m->stream));
+  k_icp_bounds<<<grid_for(n, 256, m->sm_count * 4), 256, 0, m->stream>>>(p, n, x.misc.p);
+  m->launches++;
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(x.h_misc.p, x.misc.p, sizeof(unsigned) * 7, cudaMemcpyDeviceToHost, m->stream));
+  CU(cudaStreamSynchronize(m->stream));
+  for (int a = 0; a < 3; ++a) { lo[a] = icp_fkey(x.h_misc.p[a]); hi[a] = icp_fkey(x.h_misc.p[3 + a]); }
+  *n_fin = (int)x.h_misc.p[6];
+  return 0;
+}
+
+// The grid index over the target t[0, n): *n_fin finite points (0: nothing more is built), the grid *g over their box,
+// the finite points sorted by cell into x.sorted (their original indices in x.vals_b), CSR offsets and coarse boxes.
+static int icp_index(flb_map* m, IcpIndex& x, const float4* t, int n, IcpGrid* g, int* n_fin) {
+  float lo[3], hi[3];
+  if (icp_bounds(m, x, t, n, lo, hi, n_fin)) return 1;
+  const int nf = *n_fin;
+  if (nf == 0) return 0;
+  *g = icp_grid(lo, hi, nf);
+  const unsigned n_cells = (unsigned)g->gx * g->gy * g->gz;
+  const int n_coarse = g->cx * g->cy * g->cz;
+  if (grow(x.cs, sizeof(int) * ((size_t)n_cells + 1), 0) || grow(x.box, sizeof(IcpBox) * (size_t)n_coarse, 0)) return 1;
+  size_t tb = x.tmp.cap;
+  k_icp_keys<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(*g, t, n, x.keys_a.p, x.vals_a.p);
+  CU(cub::DeviceRadixSort::SortPairs(x.tmp.p, tb, (const unsigned*)x.keys_a.p, x.keys_b.p, (const int*)x.vals_a.p, x.vals_b.p, n, 0, 32,
+                                     m->stream));
+  k_icp_gather<<<grid_for(nf, 256, m->sm_count * 8), 256, 0, m->stream>>>(x.vals_b.p, t, nf, x.sorted.p);
+  k_icp_cell_start<<<grid_for(nf + 1, 256, m->sm_count * 8), 256, 0, m->stream>>>(x.keys_b.p, nf, n_cells, x.cs.p);
+  k_icp_coarse_boxes<<<grid_for(n_coarse, 8, m->sm_count * 8), 256, 0, m->stream>>>(x.sorted.p, x.cs.p, n_coarse, x.box.p);
+  m->launches += 4 + 5;   // + the radix sort's kernels
+  CU(cudaGetLastError());
+  return 0;
+}
+
+// The queries' visiting order: the keys the caller's key kernel wrote to x.keys_a (x.vals_a the identity), sorted into
+// x.order.
+static int icp_order(flb_map* m, IcpIndex& x, int n_s) {
+  size_t tb = x.tmp.cap;
+  CU(cub::DeviceRadixSort::SortPairs(x.tmp.p, tb, (const unsigned*)x.keys_a.p, x.keys_b.p, (const int*)x.vals_a.p, x.order.p, n_s, 0, 32,
+                                     m->stream));
+  m->launches += 5;   // the radix sort's kernels
+  CU(cudaGetLastError());
+  return 0;
+}
+
+// k_reduce over n elements into out[0..K); the caller copies and synchronises.
+template <int K, class Op>
+static int icp_reduce(flb_map* m, IcpIndex& x, int n, const Op& op, double* out) {
+  k_reduce<K, Op><<<m->sm_count * 2, 256, 0, m->stream>>>(n, op, x.partials.p, x.misc.p + ICP_MISC_COUNTER, out);
+  m->launches++;
+  CU(cudaGetLastError());
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------ host algebra
@@ -177,17 +196,19 @@ static double icp_det3(const double M[9]) {
   return M[0] * (M[4] * M[8] - M[5] * M[7]) - M[1] * (M[3] * M[8] - M[5] * M[6]) + M[2] * (M[3] * M[7] - M[4] * M[6]);
 }
 
-// TransformationEstimationSVD (Umeyama, no scaling) from the sums: H = Σ (t - μt)(s - μs)^T = U S V^T,
-// R = U diag(1, 1, det U det V < 0 ? -1 : 1) V^T, t = μt - R μs, cast to a float row-major 4x4.
-static void icp_rigid(const IcpSums& s, float T[16]) {
-  double U[9], sv[3], V[9], R[9];
-  icp_svd3(s.h, U, sv, V);
+// TransformationEstimationSVD (Umeyama, no scaling) from the sums S (the pairs record, then H = Σ (t - μt)(s - μs)^T):
+// μ = Σ / count as the cross-product op forms it, H = U S V^T, R = U diag(1, 1, det U det V < 0 ? -1 : 1) V^T,
+// t = μt - R μs, cast to a float row-major 4x4.
+static void icp_rigid(const double* S, float T[16]) {
+  double mu_s[3], mu_t[3], U[9], sv[3], V[9], R[9];
+  for (int a = 0; a < 3; ++a) { mu_s[a] = S[2 + a] / S[0]; mu_t[a] = S[5 + a] / S[0]; }
+  icp_svd3(S + 8, U, sv, V);
   const double d3 = icp_det3(U) * icp_det3(V) < 0 ? -1.0 : 1.0;
   for (int r = 0; r < 3; ++r)
     for (int c = 0; c < 3; ++c) R[3 * r + c] = U[3 * r + 0] * V[3 * c + 0] + U[3 * r + 1] * V[3 * c + 1] + d3 * U[3 * r + 2] * V[3 * c + 2];
   for (int r = 0; r < 3; ++r) {
     for (int c = 0; c < 3; ++c) T[4 * r + c] = (float)R[3 * r + c];
-    T[4 * r + 3] = (float)(s.mu_t[r] - (R[3 * r] * s.mu_s[0] + R[3 * r + 1] * s.mu_s[1] + R[3 * r + 2] * s.mu_s[2]));
+    T[4 * r + 3] = (float)(mu_t[r] - (R[3 * r] * mu_s[0] + R[3 * r + 1] * mu_s[1] + R[3 * r + 2] * mu_s[2]));
   }
   T[12] = T[13] = T[14] = 0.f;
   T[15] = 1.f;
@@ -229,30 +250,44 @@ static int icp_converged(const flb_icp_config& cfg, int iterations, const float 
 }
 
 // ------------------------------------------------------------------------------------------------ device passes
+constexpr int ICP_SUM_WORDS = 17;   // the pairs record (8), then the cross products (9)
+
+// Scratch that follows the sizes of the two selections.
+static int icp_scratch(flb_map* m, KfWork& k, int n_s, int n_t, bool pre) {
+  IcpWork& w = k.icp;
+  const size_t ps = sizeof(float4) * (size_t)n_s;
+  if (icp_index_scratch(m, k.index, n_s, n_t, 0) || kf_grow(w.src_raw, ps) || (pre && kf_grow(w.src, ps)) || kf_grow(w.x, ps) ||
+      kf_grow(w.tgt, sizeof(float4) * (size_t)n_t) || kf_grow(w.corr, sizeof(int) * (size_t)n_s) ||
+      kf_grow(w.corr_d2, sizeof(float) * (size_t)n_s) || grow(w.sums, sizeof(double) * ICP_SUM_WORDS, 0) ||
+      grow(w.h_sums, sizeof(double) * ICP_SUM_WORDS, 0))
+    return 1;
+  return 0;
+}
+
 // One exact 1-NN pass: q = xf(in[i]) into w.x, nearest target into w.corr / w.corr_d2.
-static int icp_nn(flb_map* m, IcpWork& w, const IcpGrid& g, const IcpXf& xf, const float4* in, int n_s) {
-  unsigned* open_n = w.misc.p + ICP_MISC_OPEN;
+static int icp_nn(flb_map* m, KfWork& k, const IcpGrid& g, const IcpXf& xf, const float4* in, int n_s) {
+  IcpIndex& x = k.index;
+  IcpWork& w = k.icp;
+  unsigned* open_n = x.misc.p + ICP_MISC_OPEN;
   CU(cudaMemsetAsync(open_n, 0, sizeof(unsigned), m->stream));
-  k_icp_nn<<<grid_for(n_s, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, xf, w.order.p, n_s, in, w.x.p, w.sorted.p, w.cs.p, w.corr.p,
-                                                                      w.corr_d2.p, w.open.p, (int*)open_n);
-  k_icp_nn_far<<<m->sm_count * 8, 256, 0, m->stream>>>(g, w.open.p, (const int*)open_n, w.x.p, w.sorted.p, w.cs.p, w.box.p, w.corr.p,
+  k_icp_nn<<<grid_for(n_s, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, xf, x.order.p, n_s, in, w.x.p, x.sorted.p, x.cs.p, w.corr.p,
+                                                                      w.corr_d2.p, x.open.p, (int*)open_n);
+  k_icp_nn_far<<<m->sm_count * 8, 256, 0, m->stream>>>(g, x.open.p, (const int*)open_n, w.x.p, x.sorted.p, x.cs.p, x.box.p, w.corr.p,
                                                        w.corr_d2.p);
   m->launches += 2;
   CU(cudaGetLastError());
   return 0;
 }
 
-// Both reductions over the pairs of the last pass and the copy of their record; the caller synchronises.
-static int icp_reduce(flb_map* m, IcpWork& w, int n_s, double max_d2, bool cross) {
-  unsigned* counter = w.misc.p + ICP_MISC_COUNTER;
-  const int blocks = m->sm_count * 2;
-  for (int phase = 0; phase < (cross ? 2 : 1); ++phase) {
-    k_icp_reduce<<<blocks, 256, 0, m->stream>>>(phase, n_s, w.corr.p, w.corr_d2.p, w.x.p, w.tgt.p, max_d2, w.partials.p, counter,
-                                                w.sums.p);
-    m->launches++;
-  }
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(w.h_sums.p, w.sums.p, sizeof(IcpSums), cudaMemcpyDeviceToHost, m->stream));
+// The sums over the pairs of the last pass (with cross: also the cross products) and the copy of their record; the
+// caller synchronises.
+static int icp_sums(flb_map* m, KfWork& k, int n_s, double max_d2, bool cross) {
+  IcpWork& w = k.icp;
+  const IcpPairsOp pairs{w.corr.p, w.corr_d2.p, w.x.p, w.tgt.p, max_d2};
+  if (icp_reduce<8>(m, k.index, n_s, pairs, w.sums.p) ||
+      (cross && icp_reduce<9>(m, k.index, n_s, IcpCrossOp{pairs, w.sums.p}, w.sums.p + 8)))
+    return 1;
+  CU(cudaMemcpyAsync(w.h_sums.p, w.sums.p, sizeof(double) * ICP_SUM_WORDS, cudaMemcpyDeviceToHost, m->stream));
   return 0;
 }
 
@@ -299,9 +334,9 @@ extern "C" int flb_keyframes_icp(flb_keyframes* k, const int* src_ids, int n_src
   }
   flb_map* m = k->map;
   CU(cudaSetDevice(m->cfg.device));
-  IcpWork* wp = nullptr;
-  if (icp_work(m, &wp) || icp_scratch(m, *wp, n_s, n_t, src_pre_pose6 != nullptr)) return 1;
-  IcpWork& w = *wp;
+  if (kf_work(m) || icp_scratch(m, *m->kfw, n_s, n_t, src_pre_pose6 != nullptr)) return 1;
+  KfWork& kw = *m->kfw;
+  IcpWork& w = kw.icp;
 
   // the two loop sub-maps (loopFindNearKeyframes, :918-920), then cureKeyframeCloud = transformPointCloud(.., &com)
   std::vector<KfSeg> segs;
@@ -316,43 +351,18 @@ extern "C" int flb_keyframes_icp(flb_keyframes* k, const int* src_ids, int n_src
     S = w.src.p;
   }
 
-  // the target's finite box and count
-  const unsigned init[ICP_MISC_WORDS] = {~0u, ~0u, ~0u};
-  memcpy(w.h_misc.p, init, sizeof(init));
-  CU(cudaMemcpyAsync(w.misc.p, w.h_misc.p, sizeof(init), cudaMemcpyHostToDevice, m->stream));
-  k_icp_bounds<<<grid_for(n_t, 256, m->sm_count * 4), 256, 0, m->stream>>>(w.tgt.p, n_t, w.misc.p);
-  m->launches++;
-  CU(cudaGetLastError());
-  CU(cudaMemcpyAsync(w.h_misc.p, w.misc.p, sizeof(unsigned) * 7, cudaMemcpyDeviceToHost, m->stream));
-  CU(cudaStreamSynchronize(m->stream));
-  const int n_fin = (int)w.h_misc.p[6];
+  // the target's index, then the source's visiting order
+  IcpGrid g{};
+  int n_fin = 0;
+  if (icp_index(m, kw.index, w.tgt.p, n_t, &g, &n_fin)) return 1;
   if (n_fin == 0) {   // every target point dropped by KdTreeFLANN: initCompute fails
     icp_no_pairs(n_s, out_corr_index, out_corr_d2);
     *out = res;
     return 0;
   }
-  float lo[3], hi[3];
-  for (int a = 0; a < 3; ++a) { lo[a] = icp_fkey(w.h_misc.p[a]); hi[a] = icp_fkey(w.h_misc.p[3 + a]); }
-  const IcpGrid g = icp_grid(lo, hi, n_fin);
-  const unsigned n_cells = (unsigned)g.gx * g.gy * g.gz;
-  const int n_coarse = g.cx * g.cy * g.cz;
-  if (grow(w.cs, sizeof(int) * ((size_t)n_cells + 1), 0) || grow(w.box, sizeof(IcpBox) * (size_t)n_coarse, 0)) return 1;
-
-  // the index: finite target points sorted by cell, CSR offsets, coarse boxes; the source's visiting order
-  const int gt = grid_for(n_t, 256, m->sm_count * 8), gs = grid_for(n_s, 256, m->sm_count * 8);
-  size_t tb = w.tmp.cap;
-  k_icp_keys<<<gt, 256, 0, m->stream>>>(g, w.tgt.p, n_t, w.keys_a.p, w.vals_a.p);
-  CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)w.keys_a.p, w.keys_b.p, (const int*)w.vals_a.p, w.vals_b.p, n_t, 0, 32,
-                                     m->stream));
-  k_icp_gather<<<grid_for(n_fin, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.vals_b.p, w.tgt.p, n_fin, w.sorted.p);
-  k_icp_cell_start<<<grid_for(n_fin + 1, 256, m->sm_count * 8), 256, 0, m->stream>>>(w.keys_b.p, n_fin, n_cells, w.cs.p);
-  k_icp_coarse_boxes<<<grid_for(n_coarse, 8, m->sm_count * 8), 256, 0, m->stream>>>(w.sorted.p, w.cs.p, n_coarse, w.box.p);
-  k_icp_keys<<<gs, 256, 0, m->stream>>>(g, S, n_s, w.keys_a.p, w.vals_a.p);
-  tb = w.tmp.cap;
-  CU(cub::DeviceRadixSort::SortPairs(w.tmp.p, tb, (const unsigned*)w.keys_a.p, w.keys_b.p, (const int*)w.vals_a.p, w.order.p, n_s, 0, 32,
-                                     m->stream));
-  m->launches += 6 + 2 * 5;   // + the radix sorts' kernels
-  CU(cudaGetLastError());
+  k_icp_keys<<<grid_for(n_s, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, S, n_s, kw.index.keys_a.p, kw.index.vals_a.p);
+  m->launches++;
+  if (icp_order(m, kw.index, n_s)) return 1;
 
   // the iterations (icp.hpp computeTransformation)
   const double max_d2 = cfg->max_correspondence_distance * cfg->max_correspondence_distance;
@@ -362,18 +372,18 @@ extern "C" int flb_keyframes_icp(flb_keyframes* k, const int* src_ids, int n_src
   double prev_mse = DBL_MAX;
   for (int it = 0;; ++it) {
     // input_transformed <- T_{k-1} * input_transformed, fused into the pass (iteration 0 reads the source itself)
-    if (icp_nn(m, w, g, icp_xf(T, it > 0), it == 0 ? S : w.x.p, n_s) || icp_reduce(m, w, n_s, max_d2, true)) return 1;
+    if (icp_nn(m, kw, g, icp_xf(T, it > 0), it == 0 ? S : w.x.p, n_s) || icp_sums(m, kw, n_s, max_d2, true)) return 1;
     CU(cudaStreamSynchronize(m->stream));
-    const IcpSums sm = *w.h_sums.p;
-    res.n_correspondences = (int)sm.n;
-    if (sm.n < 3) {   // min_number_correspondences_
+    const double* sm = w.h_sums.p;
+    res.n_correspondences = (int)sm[0];
+    if (sm[0] < 3) {   // min_number_correspondences_
       res.state = FLB_ICP_NO_CORRESPONDENCES;
       break;
     }
     icp_rigid(sm, T);
     icp_mul4(T, final_T, final_T);
     res.iterations = it + 1;
-    res.state = icp_converged(*cfg, res.iterations, T, sm.n, sm.d2, &prev_mse);
+    res.state = icp_converged(*cfg, res.iterations, T, sm[0], sm[1], &prev_mse);
     if (res.state != FLB_ICP_NOT_CONVERGED) {
       res.converged = 1;
       break;
@@ -384,10 +394,10 @@ extern "C" int flb_keyframes_icp(flb_keyframes* k, const int* src_ids, int n_src
   if (out_corr_d2) CU(cudaMemcpyAsync(out_corr_d2, w.corr_d2.p, sizeof(float) * (size_t)n_s, cudaMemcpyDeviceToHost, m->stream));
 
   // getFitnessScore(): the original source transformed once by final, every finite point's nearest d², no cut
-  if (icp_nn(m, w, g, icp_xf(final_T, true), S, n_s) || icp_reduce(m, w, n_s, DBL_MAX, false)) return 1;
+  if (icp_nn(m, kw, g, icp_xf(final_T, true), S, n_s) || icp_sums(m, kw, n_s, DBL_MAX, false)) return 1;
   CU(cudaStreamSynchronize(m->stream));
-  const IcpSums fs = *w.h_sums.p;
-  res.fitness_score = fs.n > 0 ? fs.d2 / fs.n : DBL_MAX;
+  const double* fs = w.h_sums.p;
+  res.fitness_score = fs[0] > 0 ? fs[1] / fs[0] : DBL_MAX;
   *out = res;
   return 0;
 }

@@ -1,9 +1,14 @@
 // icp_kernels.cuh — the loop-closure registration of performLoopClosure (laserMapping.cpp:946-974,
-// pcl::IterativeClosestPoint<PointType, PointType>) between two sub-maps assembled from the key-frame store:
-//   an index over the target built once per call (finite points sorted by the cell of a uniform grid, CSR cell offsets,
-//   per-coarse-cell point boxes), an exact 1-NN pass per iteration (thread-per-query rings over the fine cells, the few
-//   open queries finished warp-per-query over the coarse cells, nearest ring first, pruned by box distance), and two
-//   fixed-order double reductions per iteration (count and means, then the demeaned cross products).
+// pcl::IterativeClosestPoint<PointType, PointType>) between two sub-maps assembled from the key-frame store, and the
+// pieces flb_keyframes_fricp (fricp_kernels.cuh) shares with it:
+//   the grid index over a float target, built once per call (finite points sorted by the cell of a uniform grid, CSR
+//   cell offsets, per-coarse-cell point boxes);
+//   the two search walks over it, generic in the query's precision: fine rings 0..ICP_RINGS thread-per-query
+//   (icp_fine_rings) and coarse rings nearest first, pruned by box distance, for the queries the fine rings leave open
+//   (icp_coarse_rings, warp- or thread-per-query);
+//   the fixed-order double reduction k_reduce.
+// The loop ICP runs an exact 1-NN pass per iteration (k_icp_nn, k_icp_nn_far) and two reductions (the pairs' count and
+// sums, then the demeaned cross products).
 // The TU is compiled with -fmad=false: the distance (dx*dx + dy*dy) + dz*dz and the affines round after every operation,
 // as the reference's FLANN L2_Simple and transformPointCloud do.  Tie rule of the 1-NN: the smaller float d², then the
 // lower target index (the position in the assembled target), so the result does not depend on the visiting order.
@@ -13,8 +18,7 @@
 namespace flb {
 
 constexpr int ICP_C = 8, ICP_C3 = ICP_C * ICP_C * ICP_C;   // fine cells per coarse-cell edge / per coarse cell
-constexpr int ICP_RINGS = 2;                                // fine rings a thread searches before the warp path takes over
-constexpr int ICP_RED = 9;                                  // doubles per reduction record
+constexpr int ICP_RINGS = 2;                                // fine rings a thread searches before the coarse walk takes over
 
 // The target's grid: fine cells of edge e from the origin (the finite minimum); gx..gz are multiples of ICP_C.  Fine
 // cell (ix, iy, iz) has key coarse * ICP_C3 + local, so every coarse cell's points are one range of the sorted target.
@@ -28,11 +32,6 @@ struct IcpGrid {
 struct IcpBox {
   float lo[3], hi[3];
   int n, pad;
-};
-
-// count, Σd² and the means of source and target over the pairs (phase 0); Σ (t - μt)(s - μs)ᵀ row-major (phase 1)
-struct IcpSums {
-  double n, d2, mu_s[3], mu_t[3], h[9];
 };
 
 // A float affine (row-major 3x4) applied as transformPointCloud does: ((m0 x + m1 y) + m2 z) + m3.
@@ -181,54 +180,56 @@ __global__ void __launch_bounds__(256) k_icp_coarse_boxes(const float4* __restri
   }
 }
 
-// ------------------------------------------------------------------------------------------------ exact 1-NN
-// Thread per query, queries in source-cell order (order[t]): q = xf(in[i]) is written to out[i] (in == out allowed), then
-// fine rings 0..ICP_RINGS, each cell pruned by its box.  A query is done when the next ring cannot hold anything closer;
-// otherwise its partial result is kept and its index appended to the open list for k_icp_nn_far.  Results by source
-// index: idx[i] = the nearest target's original index (-1 for a non-finite query), d2[i] its float d².
-__global__ void __launch_bounds__(256) k_icp_nn(IcpGrid g, IcpXf xf, const int* __restrict__ order, int n, const float4* in, float4* out,
-                                               const float4* __restrict__ pts, const int* __restrict__ cs, int* __restrict__ idx,
-                                               float* __restrict__ d2, int* __restrict__ open_list, int* __restrict__ open_n) {
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
-    const int i = order[t];
-    float4 q = in[i];
-    if (xf.apply) {
-      const float* m = xf.m;
-      q = make_float4(m[0] * q.x + m[1] * q.y + m[2] * q.z + m[3], m[4] * q.x + m[5] * q.y + m[6] * q.z + m[7],
-                      m[8] * q.x + m[9] * q.y + m[10] * q.z + m[11], q.w);
-    }
-    out[i] = q;
-    if (!icp_finite(q)) { idx[i] = -1; d2[i] = INFINITY; continue; }
-    const int c[3] = {icp_cell1(q.x, g.ox, g.inv_e, g.gx), icp_cell1(q.y, g.oy, g.inv_e, g.gy), icp_cell1(q.z, g.oz, g.inv_e, g.gz)};
-    const int dims[3] = {g.gx, g.gy, g.gz};
-    float best = INFINITY;
-    int bi = INT_MAX;
-    bool open = true;
-    for (int r = 0; r <= ICP_RINGS + 1; ++r) {
-      if (r > 0 && icp_ring_done(icp_ring_lb(g, q, c, dims, 1, r), best)) { open = false; break; }
-      if (r == ICP_RINGS + 1) break;
-      for (int dz = -r; dz <= r; ++dz) {
-        const int iz = c[2] + dz;
-        if (iz < 0 || iz >= g.gz) continue;
-        for (int dy = -r; dy <= r; ++dy) {
-          const int iy = c[1] + dy;
-          if (iy < 0 || iy >= g.gy) continue;
-          const bool face = dz == -r || dz == r || dy == -r || dy == r;
-          for (int dx = -r; dx <= r; dx += (face ? 1 : 2 * r)) {   // interior rows: only the two x faces
-            const int ix = c[0] + dx;
-            if (ix >= 0 && ix < g.gx && icp_box_lb2(g, q, ix, iy, iz, 1) <= best) {
-              const unsigned k = icp_key(g, ix, iy, iz);
-              icp_scan(pts, __ldg(&cs[k]), __ldg(&cs[k + 1]), q, best, bi);
-            }
-            if (r == 0) break;
-          }
+// ------------------------------------------------------------------------------------------------ search walks
+// The loop ICP's query: float coordinates and d², every bound in float, a ring closed with a 1e-6 relative margin in
+// double.  flb_keyframes_fricp's double query (FrQuery, fricp_kernels.cuh) has the same members.
+struct IcpQuery {
+  using real = float;
+  float4 q;
+  __device__ void cell(const IcpGrid& g, int* c) const {
+    c[0] = icp_cell1(q.x, g.ox, g.inv_e, g.gx);
+    c[1] = icp_cell1(q.y, g.oy, g.inv_e, g.gy);
+    c[2] = icp_cell1(q.z, g.oz, g.inv_e, g.gz);
+  }
+  __device__ float cell_lb2(const IcpGrid& g, int ix, int iy, int iz) const { return icp_box_lb2(g, q, ix, iy, iz, 1); }
+  __device__ float box_lb2(const IcpGrid&, const IcpBox& b) const {
+    const float dx = fmaxf(fmaxf(b.lo[0] - q.x, q.x - b.hi[0]), 0.f), dy = fmaxf(fmaxf(b.lo[1] - q.y, q.y - b.hi[1]), 0.f);
+    const float dz = fmaxf(fmaxf(b.lo[2] - q.z, q.z - b.hi[2]), 0.f);
+    return (dx * dx + dy * dy) + dz * dz;
+  }
+  __device__ bool ring_done(const IcpGrid& g, const int* c, const int* dims, int span, int r, float best) const {
+    return icp_ring_done(icp_ring_lb(g, q, c, dims, span, r), best);
+  }
+  __device__ static bool beats(float lb2, float best) { return lb2 <= best; }
+};
+
+// Fine rings 0..ICP_RINGS around the query's cell (interior rows only at their two x faces); every cell whose bound can
+// beat best goes to visit(key), which may lower best.  Returns whether the query closed: the next ring cannot hold
+// anything closer than best.
+template <class Q, class Visit>
+__device__ __forceinline__ bool icp_fine_rings(const IcpGrid& g, const Q& q, const typename Q::real& best, Visit visit) {
+  int c[3];
+  q.cell(g, c);
+  const int dims[3] = {g.gx, g.gy, g.gz};
+  for (int r = 0; r <= ICP_RINGS + 1; ++r) {
+    if (r > 0 && q.ring_done(g, c, dims, 1, r, best)) return true;
+    if (r == ICP_RINGS + 1) break;
+    for (int dz = -r; dz <= r; ++dz) {
+      const int iz = c[2] + dz;
+      if (iz < 0 || iz >= g.gz) continue;
+      for (int dy = -r; dy <= r; ++dy) {
+        const int iy = c[1] + dy;
+        if (iy < 0 || iy >= g.gy) continue;
+        const bool face = dz == -r || dz == r || dy == -r || dy == r;
+        for (int dx = -r; dx <= r; dx += (face ? 1 : 2 * r)) {   // interior rows: only the two x faces
+          const int ix = c[0] + dx;
+          if (ix >= 0 && ix < g.gx && Q::beats(q.cell_lb2(g, ix, iy, iz), best)) visit(icp_key(g, ix, iy, iz));
+          if (r == 0) break;
         }
       }
     }
-    idx[i] = bi;
-    d2[i] = best;
-    if (open) open_list[atomicAdd(open_n, 1)] = i;
   }
+  return false;
 }
 
 // The cells of Chebyshev ring R around c clipped to the grid [0, dims): t-th of *count.  Faces: z = c-R, z = c+R (full
@@ -266,103 +267,132 @@ struct IcpShell {
   }
 };
 
-// Warp per open query: coarse rings from the query's coarse cell, nearest ring first, until a ring cannot hold anything
-// closer.  A coarse cell is visited when its point box can beat the warp's best; its non-empty fine cells are then
-// pruned by their own boxes and scanned by the lanes.  Starts from the thread path's partial result.
+// Coarse rings from the query's coarse cell, nearest ring first, until a ring cannot hold anything closer than best
+// (every query closes).  A coarse cell whose point box can beat best goes to visit(id), which may lower best.  W = 32:
+// warp per query, each lane tests one cell of the ring, and the warp visits the ballot's cells in lane order, each
+// tested again against the best the earlier visits left (the visit merges the lanes' bests); W = 1: thread per query.
+template <int W, class Q, class Visit>
+__device__ __forceinline__ void icp_coarse_rings(const IcpGrid& g, const IcpBox* __restrict__ box, const Q& q,
+                                                 const typename Q::real& best, Visit visit) {
+  int c[3];
+  q.cell(g, c);
+  for (int a = 0; a < 3; ++a) c[a] /= ICP_C;
+  const int dims[3] = {g.cx, g.cy, g.cz};
+  const int lane = W == 1 ? 0 : (int)(threadIdx.x & 31);
+  for (int R = 0;; ++R) {
+    if (R > 0 && q.ring_done(g, c, dims, ICP_C, R, best)) return;
+    IcpShell sh;
+    sh.init(c, dims, R);
+    const int tot = sh.total();
+    for (int base = 0; base < tot; base += W) {
+      int cc = -1;
+      typename Q::real lb2 = INFINITY;
+      if (base + lane < tot) {
+        int o[3];
+        sh.cell(base + lane, o);
+        const int id = (o[2] * g.cy + o[1]) * g.cx + o[0];
+        const IcpBox b = box[id];
+        if (b.n > 0) {
+          lb2 = q.box_lb2(g, b);
+          if (Q::beats(lb2, best)) cc = id;
+        }
+      }
+      if constexpr (W == 1) {
+        if (cc >= 0) visit(cc);
+      } else {
+        unsigned mask = __ballot_sync(0xffffffffu, cc >= 0);
+        while (mask) {
+          const int src = __ffs(mask) - 1;
+          mask &= mask - 1;
+          const int id = __shfl_sync(0xffffffffu, cc, src);
+          if (!Q::beats(__shfl_sync(0xffffffffu, lb2, src), best)) continue;   // best improved since the ballot
+          visit(id);
+        }
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ exact 1-NN
+// Thread per query, queries in source-cell order (order[t]): q = xf(in[i]) is written to out[i] (in == out allowed), then
+// the fine rings, each cell pruned by its box.  A query the rings do not close keeps its partial result and its index
+// goes to the open list for k_icp_nn_far.  Results by source index: idx[i] = the nearest target's original index (-1 for
+// a non-finite query), d2[i] its float d².
+__global__ void __launch_bounds__(256) k_icp_nn(IcpGrid g, IcpXf xf, const int* __restrict__ order, int n, const float4* in, float4* out,
+                                               const float4* __restrict__ pts, const int* __restrict__ cs, int* __restrict__ idx,
+                                               float* __restrict__ d2, int* __restrict__ open_list, int* __restrict__ open_n) {
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+    const int i = order[t];
+    float4 q = in[i];
+    if (xf.apply) {
+      const float* m = xf.m;
+      q = make_float4(m[0] * q.x + m[1] * q.y + m[2] * q.z + m[3], m[4] * q.x + m[5] * q.y + m[6] * q.z + m[7],
+                      m[8] * q.x + m[9] * q.y + m[10] * q.z + m[11], q.w);
+    }
+    out[i] = q;
+    if (!icp_finite(q)) { idx[i] = -1; d2[i] = INFINITY; continue; }
+    float best = INFINITY;
+    int bi = INT_MAX;
+    const bool closed = icp_fine_rings(g, IcpQuery{q}, best, [&](unsigned k) {
+      icp_scan(pts, __ldg(&cs[k]), __ldg(&cs[k + 1]), q, best, bi);
+    });
+    idx[i] = bi;
+    d2[i] = best;
+    if (!closed) open_list[atomicAdd(open_n, 1)] = i;
+  }
+}
+
+// Warp per open query over the coarse rings, starting from the thread path's partial result.  A visited coarse cell's
+// non-empty fine cells are pruned by their own boxes and scanned by the lanes.
 __global__ void __launch_bounds__(256) k_icp_nn_far(IcpGrid g, const int* __restrict__ open_list, const int* __restrict__ open_n,
                                                    const float4* __restrict__ xq, const float4* __restrict__ pts,
                                                    const int* __restrict__ cs, const IcpBox* __restrict__ box, int* __restrict__ idx,
                                                    float* __restrict__ d2) {
   const int lane = threadIdx.x & 31;
   const int n_open = *open_n;
-  const int dims[3] = {g.cx, g.cy, g.cz};
   for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < n_open; w += (gridDim.x * blockDim.x) >> 5) {
     const int i = open_list[w];
     const float4 q = xq[i];
     float best = d2[i];
     int bi = idx[i];
-    const int c[3] = {icp_cell1(q.x, g.ox, g.inv_e, g.gx) / ICP_C, icp_cell1(q.y, g.oy, g.inv_e, g.gy) / ICP_C,
-                      icp_cell1(q.z, g.oz, g.inv_e, g.gz) / ICP_C};
-    for (int R = 0;; ++R) {
-      if (R > 0 && icp_ring_done(icp_ring_lb(g, q, c, dims, ICP_C, R), best)) break;
-      IcpShell sh;
-      sh.init(c, dims, R);
-      const int tot = sh.total();
-      for (int base = 0; base < tot; base += 32) {
-        int cc = -1;
-        float lb2 = INFINITY;
-        if (base + lane < tot) {
-          int o[3];
-          sh.cell(base + lane, o);
-          const int id = (o[2] * g.cy + o[1]) * g.cx + o[0];
-          const IcpBox b = box[id];
-          if (b.n > 0) {
-            const float dx = fmaxf(fmaxf(b.lo[0] - q.x, q.x - b.hi[0]), 0.f), dy = fmaxf(fmaxf(b.lo[1] - q.y, q.y - b.hi[1]), 0.f);
-            const float dz = fmaxf(fmaxf(b.lo[2] - q.z, q.z - b.hi[2]), 0.f);
-            lb2 = (dx * dx + dy * dy) + dz * dz;
-            if (lb2 <= best) cc = id;
-          }
-        }
-        unsigned mask = __ballot_sync(0xffffffffu, cc >= 0);
-        while (mask) {
-          const int src = __ffs(mask) - 1;
-          mask &= mask - 1;
-          const int id = __shfl_sync(0xffffffffu, cc, src);
-          if (__shfl_sync(0xffffffffu, lb2, src) > best) continue;   // best improved since the ballot
-          const int bx = (id % g.cx) * ICP_C, by = ((id / g.cx) % g.cy) * ICP_C, bz = (id / (g.cx * g.cy)) * ICP_C;
-          for (int l = lane; l < ICP_C3; l += 32) {
-            const int k = id * ICP_C3 + l;
-            const int s = __ldg(&cs[k]), e = __ldg(&cs[k + 1]);
-            if (s < e && icp_box_lb2(g, q, bx + l % ICP_C, by + (l / ICP_C) % ICP_C, bz + l / (ICP_C * ICP_C), 1) <= best)
-              icp_scan(pts, s, e, q, best, bi);
-          }
-          for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            icp_take(ob, oi, best, bi);
-          }
-        }
+    icp_coarse_rings<32>(g, box, IcpQuery{q}, best, [&](int id) {
+      const int bx = (id % g.cx) * ICP_C, by = ((id / g.cx) % g.cy) * ICP_C, bz = (id / (g.cx * g.cy)) * ICP_C;
+      for (int l = lane; l < ICP_C3; l += 32) {
+        const int k = id * ICP_C3 + l;
+        const int s = __ldg(&cs[k]), e = __ldg(&cs[k + 1]);
+        if (s < e && icp_box_lb2(g, q, bx + l % ICP_C, by + (l / ICP_C) % ICP_C, bz + l / (ICP_C * ICP_C), 1) <= best)
+          icp_scan(pts, s, e, q, best, bi);
       }
-    }
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        icp_take(ob, oi, best, bi);
+      }
+    });
     if (lane == 0) { idx[i] = bi; d2[i] = best; }
   }
 }
 
 // ------------------------------------------------------------------------------------------------ reductions
-// Fixed-order double sums over the pairs (idx[i] >= 0 and (double)d2[i] <= max_d2): block b takes a fixed contiguous
-// range of sources, each thread sums its strided share in index order, the block reduces in a fixed tree, and the last
-// block to finish sums the block partials in block order.  Phase 0: count, Σd², means of source and target (into out);
-// phase 1 (after phase 0, reading its means): the 9 cross products.  Run-to-run bit-identical for a given grid.
-__global__ void __launch_bounds__(256) k_icp_reduce(int phase, int n, const int* __restrict__ idx, const float* __restrict__ d2,
-                                                   const float4* __restrict__ src, const float4* __restrict__ tgt, double max_d2,
-                                                   double* __restrict__ partials, unsigned* __restrict__ counter, IcpSums* out) {
-  __shared__ double sh[ICP_RED][256];
+constexpr int ICP_RED_MAX = 17;   // doubles of the widest record (flb_keyframes_fricp's step record)
+
+// Fixed-order double sums of K values per element (op(i, a) fills a[0..K) and returns whether element i counts): block b
+// takes a fixed contiguous range, each thread sums its strided share in index order, the block reduces in a fixed tree,
+// and the last block to finish sums the block partials in block order into out[0..K).  Run-to-run bit-identical for a
+// given grid.
+template <int K, class Op>
+__global__ void __launch_bounds__(256) k_reduce(int n, Op op, double* __restrict__ partials, unsigned* __restrict__ counter,
+                                               double* __restrict__ out) {
+  static_assert(K <= ICP_RED_MAX, "the partials hold ICP_RED_MAX doubles per block");
+  __shared__ double sh[K][256];
   __shared__ bool last;
-  double acc[ICP_RED];
-  for (int k = 0; k < ICP_RED; ++k) acc[k] = 0.0;
-  double ms[3] = {0, 0, 0}, mt[3] = {0, 0, 0};
-  if (phase == 1)
-    for (int a = 0; a < 3; ++a) { ms[a] = out->mu_s[a]; mt[a] = out->mu_t[a]; }
+  double acc[K], a[K];
+  for (int k = 0; k < K; ++k) acc[k] = 0.0;
   const int chunk = (n + gridDim.x - 1) / gridDim.x;
   const int b0 = blockIdx.x * chunk, b1 = min(n, b0 + chunk);
-  for (int i = b0 + threadIdx.x; i < b1; i += blockDim.x) {
-    const int j = idx[i];
-    if (j < 0) continue;
-    const float dd = d2[i];
-    if (!((double)dd <= max_d2)) continue;
-    const float4 s = src[i], t = tgt[j];
-    if (phase == 0) {
-      acc[0] += 1.0;
-      acc[1] += (double)dd;
-      acc[2] += s.x; acc[3] += s.y; acc[4] += s.z;
-      acc[5] += t.x; acc[6] += t.y; acc[7] += t.z;
-    } else {
-      const double ds[3] = {s.x - ms[0], s.y - ms[1], s.z - ms[2]}, dt[3] = {t.x - mt[0], t.y - mt[1], t.z - mt[2]};
-      for (int r = 0; r < 3; ++r)
-        for (int cc = 0; cc < 3; ++cc) acc[3 * r + cc] += dt[r] * ds[cc];
-    }
-  }
-  const int K = phase == 0 ? 8 : 9;
+  for (int i = b0 + threadIdx.x; i < b1; i += blockDim.x)
+    if (op(i, a))
+      for (int k = 0; k < K; ++k) acc[k] += a[k];
   for (int k = 0; k < K; ++k) sh[k][threadIdx.x] = acc[k];
   __syncthreads();
   for (int s = blockDim.x / 2; s > 0; s >>= 1) {
@@ -371,7 +401,7 @@ __global__ void __launch_bounds__(256) k_icp_reduce(int phase, int n, const int*
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    for (int k = 0; k < K; ++k) partials[(size_t)blockIdx.x * ICP_RED + k] = sh[k][0];
+    for (int k = 0; k < K; ++k) partials[(size_t)blockIdx.x * K + k] = sh[k][0];
     __threadfence();
     last = atomicAdd(counter, 1u) == gridDim.x - 1;
   }
@@ -380,7 +410,7 @@ __global__ void __launch_bounds__(256) k_icp_reduce(int phase, int n, const int*
   __threadfence();
   for (int k = 0; k < K; ++k) {
     double v = 0.0;
-    for (int b = threadIdx.x; b < (int)gridDim.x; b += blockDim.x) v += ((volatile double*)partials)[(size_t)b * ICP_RED + k];
+    for (int b = threadIdx.x; b < (int)gridDim.x; b += blockDim.x) v += ((volatile double*)partials)[(size_t)b * K + k];
     sh[k][threadIdx.x] = v;
   }
   __syncthreads();
@@ -390,19 +420,46 @@ __global__ void __launch_bounds__(256) k_icp_reduce(int phase, int n, const int*
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    if (phase == 0) {
-      const double cnt = sh[0][0];
-      out->n = cnt;
-      out->d2 = sh[1][0];
-      for (int a = 0; a < 3; ++a) {
-        out->mu_s[a] = cnt > 0 ? sh[2 + a][0] / cnt : 0.0;
-        out->mu_t[a] = cnt > 0 ? sh[5 + a][0] / cnt : 0.0;
-      }
-    } else {
-      for (int k = 0; k < 9; ++k) out->h[k] = sh[k][0];
-    }
+    for (int k = 0; k < K; ++k) out[k] = sh[k][0];
     *counter = 0u;
   }
 }
+
+// The pairs of a 1-NN pass (idx[i] >= 0 and (double)d2[i] <= max_d2): count, Σd², Σ source, Σ target (k_reduce<8>).
+struct IcpPairsOp {
+  const int* idx;
+  const float* d2;
+  const float4* src;
+  const float4* tgt;
+  double max_d2;
+  __device__ bool operator()(int i, double* a) const {
+    const int j = idx[i];
+    if (j < 0) return false;
+    const float dd = d2[i];
+    if (!((double)dd <= max_d2)) return false;
+    const float4 s = src[i], t = tgt[j];
+    a[0] = 1.0;
+    a[1] = (double)dd;
+    a[2] = s.x; a[3] = s.y; a[4] = s.z;
+    a[5] = t.x; a[6] = t.y; a[7] = t.z;
+    return true;
+  }
+};
+
+// Σ (t - μt)(s - μs)ᵀ row-major over the same pairs (k_reduce<9>), each mean formed as sum / count from the pairs record.
+struct IcpCrossOp {
+  IcpPairsOp pairs;
+  const double* rec;
+  __device__ bool operator()(int i, double* a) const {
+    const double n = rec[0];
+    const double ms[3] = {rec[2] / n, rec[3] / n, rec[4] / n}, mt[3] = {rec[5] / n, rec[6] / n, rec[7] / n};
+    double p[8];
+    if (!pairs(i, p)) return false;
+    const double ds[3] = {p[2] - ms[0], p[3] - ms[1], p[4] - ms[2]}, dt[3] = {p[5] - mt[0], p[6] - mt[1], p[7] - mt[2]};
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) a[3 * r + c] = dt[r] * ds[c];
+    return true;
+  }
+};
 
 }  // namespace flb

@@ -4,21 +4,50 @@
 // (saveMapService :1763-1798, the per-key-frame saver :2501-2530).  Every reader assembles its selection with one
 // k_kf_assemble launch.  Included at the end of fastlio_b200.cu after frontend_host.cuh (uses VgWork, flb_frontend).
 #pragma once
+#include "icp_kernels.cuh"
 #include "keyframe_kernels.cuh"
 #include "scan_context_kernels.cuh"
-
-struct IcpWork;                            // ICP scratch (icp_host.cuh)
-static void icp_release(IcpWork* w);
-static size_t icp_device_bytes(const IcpWork* w);
-struct FricpWork;                          // relocalisation registration scratch (fricp_host.cuh)
-static void fricp_release(FricpWork* w);
-static size_t fricp_device_bytes(const FricpWork* w);
 
 // ------------------------------------------------------------------------------------------------ map-side scratch
 // Kept with the map and only ever grown, like kf_raw / kf_in / kf_out: the readers run every kd_step key frames or on a
 // service call with selections of similar size, and cudaMalloc / cudaFree of a few hundred MB cost more than the kernels.
 // Each path allocates only the buffers it uses; flb_keyframes_info reports the total and
 // flb_map_release_keyframe_scratch frees it (e.g. after saving a map of the whole run).
+// The grid index of flb_keyframes_icp and flb_keyframes_fricp (icp_host.cuh) and the reductions' scratch.  Both calls
+// run on the map's stream and synchronise before returning, so they share it.
+struct IcpIndex {
+  DevBuf<float4> sorted;                       // sorted finite target (w = original index)
+  DevBuf<unsigned> keys_a, keys_b;             // radix-sort keys
+  DevBuf<int> vals_a, vals_b, order, open;     // radix-sort values (vals_b: the sorted original indices); source visiting
+                                               // order; open queries of the fine rings
+  DevBuf<int> cs;                              // CSR cell offsets (n_cells + 1)
+  DevBuf<IcpBox> box;                          // coarse-cell point boxes
+  DevBuf<unsigned char> tmp;                   // CUB temporary storage
+  DevBuf<double> partials;                     // reduction block partials
+  DevBuf<unsigned> misc;                       // bounds keys (6), finite count, open count, reduction counter
+  PinnedBuf<unsigned> h_misc;
+};
+
+// flb_keyframes_icp's own scratch (icp_host.cuh)
+struct IcpWork {
+  DevBuf<float4> src_raw, src, x, tgt;         // assembled source, pre-transformed source, input_transformed, target
+  DevBuf<int> corr;                            // nearest target per source
+  DevBuf<float> corr_d2;
+  DevBuf<double> sums;                         // the pairs record (8) and the cross products (9)
+  PinnedBuf<double> h_sums;
+};
+
+// flb_keyframes_fricp's own scratch (fricp_host.cuh)
+struct FricpWork {
+  DevBuf<unsigned char> raw;                   // staged source records
+  DevBuf<float4> src_raw, src, tgt_a, tgt, tgtf;   // uploaded / pre-transformed source, the two target stages, float target
+  DevBuf<double4> x, tn, sorted_d;             // normalised source, normalised target, sorted finite target (w = index)
+  DevBuf<int> pos, corr;                       // sorted position of the nearest target; its original index
+  DevBuf<double> d2, med, sort_a, sort_b;      // 1-NN d²; 7-NN medians; sort input / output of a median
+  DevBuf<double> sums;                         // reduction records
+  PinnedBuf<double> h_sums;
+};
+
 struct KfWork {
   VgWork vg;                                   // voxel grid of the sub-map / saved map
   DevBuf<float> cin, cout;                     // curvature of an assembly and of its filtered output
@@ -29,15 +58,14 @@ struct KfWork {
   PinnedBuf<ScChunk> h_chunk;                  //   and its staging
   DevBuf<unsigned> d_sc_keys;                  // Scan Context keys, SC_BINS per descriptor
   PinnedBuf<unsigned> h_sc_keys;               //   and their staging
-  IcpWork* icp = nullptr;                      // flb_keyframes_icp's sub-maps, target index and reductions
-  FricpWork* fricp = nullptr;                  // flb_keyframes_fricp's clouds, target index, medians and reductions
+  IcpIndex index;                              // the registrations' target index and reductions
+  IcpWork icp;                                 // flb_keyframes_icp's sub-maps and matches
+  FricpWork fricp;                             // flb_keyframes_fricp's clouds, matches and medians
 };
 
 static void kfw_release(KfWork* w) {
   if (!w) return;
   if (w->ev_seg) Q(cudaEventDestroy(w->ev_seg));
-  icp_release(w->icp);
-  fricp_release(w->fricp);
   delete w;
 }
 
@@ -73,9 +101,17 @@ static int kf_scratch(flb_map* m, int n, bool curv, bool filter) {
 
 static long long kf_scratch_bytes(const flb_map* m) {
   size_t b = m->kf_raw.cap + m->kf_in.cap + m->kf_out.cap;   // device bytes (the pinned staging is not counted)
-  if (const KfWork* w = m->kfw)
-    b += w->cin.cap + w->cout.cap + w->d_seg.cap + w->d_chunk.cap + w->d_sc_keys.cap + vg_device_bytes(w->vg) + icp_device_bytes(w->icp) +
-         fricp_device_bytes(w->fricp);
+  if (const KfWork* w = m->kfw) {
+    const IcpIndex& x = w->index;
+    const IcpWork& i = w->icp;
+    const FricpWork& f = w->fricp;
+    b += w->cin.cap + w->cout.cap + w->d_seg.cap + w->d_chunk.cap + w->d_sc_keys.cap + vg_device_bytes(w->vg);
+    b += x.sorted.cap + x.keys_a.cap + x.keys_b.cap + x.vals_a.cap + x.vals_b.cap + x.order.cap + x.open.cap + x.cs.cap + x.box.cap +
+         x.tmp.cap + x.partials.cap + x.misc.cap;
+    b += i.src_raw.cap + i.src.cap + i.x.cap + i.tgt.cap + i.corr.cap + i.corr_d2.cap + i.sums.cap;
+    b += f.raw.cap + f.src_raw.cap + f.src.cap + f.tgt_a.cap + f.tgt.cap + f.tgtf.cap + f.x.cap + f.tn.cap + f.sorted_d.cap + f.pos.cap +
+         f.corr.cap + f.d2.cap + f.med.cap + f.sort_a.cap + f.sort_b.cap + f.sums.cap;
+  }
   return (long long)b;
 }
 
