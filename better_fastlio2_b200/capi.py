@@ -92,6 +92,19 @@ class FricpResult(C.Structure):
 FRICP_STATUS = ["OK", "FEW_TARGET", "NO_SOURCE"]
 
 
+class SicpConfig(C.Structure):
+    _fields_ = [("p", C.c_double), ("mu", C.c_double), ("alpha", C.c_double), ("max_mu", C.c_double), ("max_icp", C.c_int),
+                ("max_outer", C.c_int), ("stop", C.c_double)]
+
+
+class SicpResult(C.Structure):
+    _fields_ = [("res_trans", C.c_double * 16), ("status", C.c_int), ("iterations", C.c_int), ("admm_iterations", C.c_int),
+                ("scale", C.c_double), ("mu_source", C.c_double * 3), ("mu_target", C.c_double * 3), ("n_source", C.c_int),
+                ("n_target", C.c_int), ("n_source_finite", C.c_int), ("n_target_finite", C.c_int), ("primal", C.c_double),
+                ("dual", C.c_double), ("stop", C.c_double), ("mu_exit", C.c_double), ("syncs", C.c_int), ("admm_blocks", C.c_int),
+                ("log_n", C.c_int)]
+
+
 class IcpResult(C.Structure):
     _fields_ = [("final_transformation", C.c_float * 16), ("converged", C.c_int), ("iterations", C.c_int), ("state", C.c_int),
                 ("n_source", C.c_int), ("n_target", C.c_int), ("n_correspondences", C.c_int), ("fitness_score", C.c_double)]
@@ -121,7 +134,7 @@ EXPORTS = [
     "flb_keyframes_download", "flb_keyframes_info", "flb_keyframes_size", "flb_map_reconstruct_from_keyframes",
     "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
     "flb_keyframes_scan_context", "flb_keyframes_scan_contexts", "flb_keyframes_icp",
-    "flb_fricp_default_config", "flb_keyframes_fricp",
+    "flb_fricp_default_config", "flb_keyframes_fricp", "flb_sicp_default_config", "flb_keyframes_sicp",
     "flb_frontend_camera_config", "flb_frontend_camera_image", "flb_frontend_points_colorize", "flb_frontend_points_to_imu",
 ]
 
@@ -225,6 +238,10 @@ def lib():
         L.flb_fricp_default_config.restype = None
         L.flb_keyframes_fricp.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, fp, vp, C.c_int, fp, fp, C.POINTER(FricpConfig),
                                           C.POINTER(FricpResult), vp, dp, dp, C.c_int]
+        L.flb_sicp_default_config.argtypes = [C.POINTER(SicpConfig)]
+        L.flb_sicp_default_config.restype = None
+        L.flb_keyframes_sicp.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, fp, vp, C.c_int, fp, fp, C.POINTER(SicpConfig),
+                                         C.POINTER(SicpResult), vp, dp, dp, C.c_int]
         _lib = L
     return _lib
 
@@ -936,6 +953,54 @@ class KeyFrameStore:
                "scale": r.scale, "mu_source": np.array(r.mu_source[:]), "mu_target": np.array(r.mu_target[:]),
                "nu_begin": r.nu_begin, "nu_end": r.nu_end, "energy": r.energy, "n_source": r.n_source, "n_target": r.n_target,
                "n_source_finite": r.n_source_finite, "n_target_finite": r.n_target_finite}
+        out = (res,)
+        if correspondences:
+            out += (idx[:n].copy(), resid[:n].copy())
+        if log:
+            out += (lg[:r.log_n].copy(),)
+        return out if len(out) > 1 else res
+
+    @staticmethod
+    def _source(src_points):
+        pts = np.ascontiguousarray(src_points, np.float32)
+        if pts.ndim != 2 or pts.shape[1] not in (3, 4, 12):
+            raise ValueError("src_points must be (n,3), (n,4) or (n,12) float32")
+        off_i = -1 if pts.shape[1] == 3 else (12 if pts.shape[1] == 4 else OFF_INTENSITY)
+        return pts, 4 * pts.shape[1], off_i
+
+    def sicp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, p=0.4, mu=10.0, alpha=1.2, max_mu=1e5,
+             max_icp=100, max_outer=100, stop=1e-5, correspondences=False, log=False, log_cap=4096):
+        """The relocaliser's Sparse ICP (regMode 7) on the device, with the clouds of fricp(): the host source, moved by
+        src_pose6 when given, onto the key frames tgt_ids each moved by tgt_pre_pose6 when given and then by its tgt_poses6
+        row.  Returns a dict (res_trans (4,4) float64, status, status_name, iterations, admm_iterations, scale, mu_source,
+        mu_target, n_source, n_target, n_source_finite, n_target_finite, primal, dual, stop, mu_exit, syncs, admm_blocks) and, in this
+        order when asked for, the last ICP iteration's matched target index (-1: none) and residual of every source point,
+        and the per-ICP-iteration log ((k, 5): ADMM iterations, primal, dual, stop, μ at exit)."""
+        pts, stride, off_i = self._source(src_points)
+        n = len(pts)
+        ids = np.ascontiguousarray(tgt_ids, np.int32).reshape(-1)
+        p6 = np.ascontiguousarray(tgt_poses6, np.float32).reshape(-1, 6)
+        if len(p6) != len(ids):
+            raise ValueError("one pose per target key frame")
+        pre = None if tgt_pre_pose6 is None else np.ascontiguousarray(tgt_pre_pose6, np.float32).reshape(6)
+        sp = None if src_pose6 is None else np.ascontiguousarray(src_pose6, np.float32).reshape(6)
+        cfg = SicpConfig(float(p), float(mu), float(alpha), float(max_mu), int(max_icp), int(max_outer), float(stop))
+        r = SicpResult()
+        idx = resid = lg = None
+        if correspondences:
+            idx = np.empty(max(n, 1), np.int32)
+            resid = np.empty(max(n, 1), np.float64)
+        if log:
+            lg = np.zeros((max(int(log_cap), 1), 5), np.float64)
+        _chk(lib().flb_keyframes_sicp(self.h, _p(pts) if n else None, n, stride, off_i, _p(sp), _p(ids) if len(ids) else None, len(ids),
+                                      _p(pre), _p(p6) if len(ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(resid), _p(lg),
+                                      int(log_cap) if log else 0))
+        res = {"res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
+               "status_name": FRICP_STATUS[r.status], "iterations": r.iterations, "admm_iterations": r.admm_iterations,
+               "scale": r.scale, "mu_source": np.array(r.mu_source[:]), "mu_target": np.array(r.mu_target[:]),
+               "n_source": r.n_source, "n_target": r.n_target, "n_source_finite": r.n_source_finite,
+               "n_target_finite": r.n_target_finite, "primal": r.primal, "dual": r.dual, "stop": r.stop, "mu_exit": r.mu_exit,
+               "syncs": r.syncs, "admm_blocks": r.admm_blocks}
         out = (res,)
         if correspondences:
             out += (idx[:n].copy(), resid[:n].copy())

@@ -137,8 +137,13 @@ static int icp_reduce(flb_map* m, IcpIndex& x, int n, const Op& op, double* out)
 
 // ------------------------------------------------------------------------------------------------ host algebra
 // One-sided Jacobi SVD of a 3x3 double matrix: A = U diag(s) V^T, s descending.  Columns of U for a zero singular value
-// are completed to an orthonormal basis (u3 = u1 x u2).
-static void icp_svd3(const double A[9], double U[9], double s[3], double V[9]) {
+// are completed to an orthonormal basis (u3 = u1 x u2).  Host and device (flb_keyframes_sicp solves it in every block of
+// its ADMM kernel): only + - * / sqrt, so with -fmad=false both sides give the same bits.  The columns are ordered by a
+// stable insertion sort written out as libstdc++'s std::sort runs it for three elements (a move to the front when the new
+// element precedes the first, else a linear insert), so host results are those of the std::sort it replaced.
+__host__ __device__ inline double icp_max(double a, double b) { return a < b ? b : a; }   // std::max
+
+__host__ __device__ static void icp_svd3(const double A[9], double U[9], double s[3], double V[9]) {
   double B[9];
   memcpy(B, A, sizeof(B));
   for (int i = 0; i < 9; ++i) V[i] = (i % 4 == 0) ? 1.0 : 0.0;
@@ -148,11 +153,11 @@ static void icp_svd3(const double A[9], double U[9], double s[3], double V[9]) {
       for (int q = p + 1; q < 3; ++q) {
         double a = 0, b = 0, c = 0;
         for (int r = 0; r < 3; ++r) { a += B[3 * r + p] * B[3 * r + p]; b += B[3 * r + q] * B[3 * r + q]; c += B[3 * r + p] * B[3 * r + q]; }
-        if (c == 0.0 || std::fabs(c) <= 1e-300) continue;
-        off = std::max(off, std::fabs(c) / std::sqrt(a * b));
+        if (c == 0.0 || fabs(c) <= 1e-300) continue;
+        off = icp_max(off, fabs(c) / sqrt(a * b));
         const double zeta = (b - a) / (2.0 * c);
-        const double t = (zeta >= 0 ? 1.0 : -1.0) / (std::fabs(zeta) + std::sqrt(1.0 + zeta * zeta));
-        const double cs = 1.0 / std::sqrt(1.0 + t * t), sn = cs * t;
+        const double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+        const double cs = 1.0 / sqrt(1.0 + t * t), sn = cs * t;
         for (int r = 0; r < 3; ++r) {
           const double bp = B[3 * r + p], bq = B[3 * r + q];
           B[3 * r + p] = cs * bp - sn * bq;
@@ -166,23 +171,32 @@ static void icp_svd3(const double A[9], double U[9], double s[3], double V[9]) {
   }
   int ord[3] = {0, 1, 2};
   double nrm[3];
-  for (int j = 0; j < 3; ++j) nrm[j] = std::sqrt(B[j] * B[j] + B[3 + j] * B[3 + j] + B[6 + j] * B[6 + j]);
-  std::sort(ord, ord + 3, [&](int x, int y) { return nrm[x] > nrm[y]; });
+  for (int j = 0; j < 3; ++j) nrm[j] = sqrt(B[j] * B[j] + B[3 + j] * B[3 + j] + B[6 + j] * B[6 + j]);
+  for (int i = 1; i < 3; ++i) {   // descending by nrm
+    const int v = ord[i];
+    int j = i;
+    if (nrm[v] > nrm[ord[0]]) {
+      for (; j > 0; --j) ord[j] = ord[j - 1];
+    } else {
+      for (; nrm[v] > nrm[ord[j - 1]]; --j) ord[j] = ord[j - 1];
+    }
+    ord[j] = v;
+  }
   double Bs[9], Vs[9];
   for (int j = 0; j < 3; ++j)
     for (int r = 0; r < 3; ++r) { Bs[3 * r + j] = B[3 * r + ord[j]]; Vs[3 * r + j] = V[3 * r + ord[j]]; }
   memcpy(V, Vs, sizeof(Vs));
   for (int j = 0; j < 3; ++j) s[j] = nrm[ord[j]];
-  const double tiny = std::max(s[0], 1e-300) * 1e-13;
+  const double tiny = icp_max(s[0], 1e-300) * 1e-13;
   for (int j = 0; j < 3; ++j)
     for (int r = 0; r < 3; ++r) U[3 * r + j] = s[j] > tiny ? Bs[3 * r + j] / s[j] : 0.0;
   if (!(s[1] > tiny)) {   // rank <= 1: any unit vector orthogonal to u1
     const double u0[3] = {U[0], U[3], U[6]};
     double w[3] = {0, 0, 0};
-    w[std::fabs(u0[0]) < 0.6 ? 0 : (std::fabs(u0[1]) < 0.6 ? 1 : 2)] = 1.0;
+    w[fabs(u0[0]) < 0.6 ? 0 : (fabs(u0[1]) < 0.6 ? 1 : 2)] = 1.0;
     const double d = w[0] * u0[0] + w[1] * u0[1] + w[2] * u0[2];
     double v[3] = {w[0] - d * u0[0], w[1] - d * u0[1], w[2] - d * u0[2]};
-    const double nv = std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    const double nv = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
     for (int r = 0; r < 3; ++r) U[3 * r + 1] = v[r] / nv;
   }
   if (!(s[2] > tiny)) {
@@ -192,7 +206,7 @@ static void icp_svd3(const double A[9], double U[9], double s[3], double V[9]) {
   }
 }
 
-static double icp_det3(const double M[9]) {
+__host__ __device__ static double icp_det3(const double M[9]) {
   return M[0] * (M[4] * M[8] - M[5] * M[7]) - M[1] * (M[3] * M[8] - M[5] * M[6]) + M[2] * (M[3] * M[7] - M[4] * M[6]);
 }
 

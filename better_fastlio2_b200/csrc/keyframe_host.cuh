@@ -48,6 +48,16 @@ struct FricpWork {
   PinnedBuf<double> h_sums;
 };
 
+// flb_keyframes_sicp's own scratch (sicp_host.cuh); its clouds, matches and index are flb_keyframes_fricp's
+struct SicpWork {
+  DevBuf<double4> q, z, c, xo2;                // per source point: match, shrunk residual, multiplier, X of the last ICP
+                                               // iteration
+  DevBuf<double> sched;                        // μ, Ba, ha per outer iteration
+  PinnedBuf<double> h_sched;
+  DevBuf<double> part, rec;                    // the ADMM kernel's block partials and its per-iteration record
+  PinnedBuf<double> h_rec;
+};
+
 struct KfWork {
   VgWork vg;                                   // voxel grid of the sub-map / saved map
   DevBuf<float> cin, cout;                     // curvature of an assembly and of its filtered output
@@ -61,6 +71,7 @@ struct KfWork {
   IcpIndex index;                              // the registrations' target index and reductions
   IcpWork icp;                                 // flb_keyframes_icp's sub-maps and matches
   FricpWork fricp;                             // flb_keyframes_fricp's clouds, matches and medians
+  SicpWork sicp;                               // flb_keyframes_sicp's ADMM state
 };
 
 static void kfw_release(KfWork* w) {
@@ -111,6 +122,8 @@ static long long kf_scratch_bytes(const flb_map* m) {
     b += i.src_raw.cap + i.src.cap + i.x.cap + i.tgt.cap + i.corr.cap + i.corr_d2.cap + i.sums.cap;
     b += f.raw.cap + f.src_raw.cap + f.src.cap + f.tgt_a.cap + f.tgt.cap + f.tgtf.cap + f.x.cap + f.tn.cap + f.sorted_d.cap + f.pos.cap +
          f.corr.cap + f.d2.cap + f.med.cap + f.sort_a.cap + f.sort_b.cap + f.sums.cap;
+    const SicpWork& s = w->sicp;
+    b += s.q.cap + s.z.cap + s.c.cap + s.xo2.cap + s.sched.cap + s.part.cap + s.rec.cap;
   }
   return (long long)b;
 }

@@ -527,6 +527,47 @@ int flb_keyframes_fricp(flb_keyframes* kf, const void* src_points, int n_src, in
                         const flb_fricp_config* cfg, flb_fricp_result* out, int* out_corr_index, double* out_resid,
                         double* out_log, int log_cap);
 
+/* ------------------------------------------------------------------------------------------------ relocalisation Sparse ICP
+ * The relocaliser's regMode 7 (Sparse ICP, SICP::point_to_point, include/FRICP-toolkit/ICP.h:275-380, with Registeration's
+ * SICP::Parameters, registeration.h:67-69, :143-146).  Source, target, the dropping of non-finite points and the
+ * normalisation are flb_keyframes_fricp's.  Each ICP iteration matches every source point X_i to its exact nearest target
+ * point Q_i (double d², equal d²: the lower target index), then runs the ADMM loop: Z = (X - Q) + C/μ shrunk by the ℓp
+ * operator, the unweighted Kabsch step onto U = (Q + Z) - C/μ, X and T moved, C += μ ((X - Q) - Z), μ *= alpha while
+ * μ < max_mu, until max |P| and Σ|ΔX|²/n are both below stop or max_outer passes.  Z and C persist across ICP iterations;
+ * μ restarts from mu.  The ICP loop ends after max_icp iterations or when max |X - X_prev| < stop.  DESIGN.md §9 states
+ * the contract and its deviations.  The whole ADMM loop runs on the device: one synchronisation per ICP iteration.  Every
+ * argument is checked before any device work; the store and the map are not modified.  The ADMM state is map-side
+ * key-frame scratch (flb_keyframes_info, flb_map_release_keyframe_scratch).  Statuses are FLB_FRICP_*; FEW_TARGET means
+ * no finite target point. */
+typedef struct flb_sicp_config {
+  double p;                            /* the ℓp exponent (0.4), in (0, 1] */
+  double mu, alpha, max_mu;            /* the penalty's start (10), growth factor (1.2, >= 1) and cap (1e5) */
+  int max_icp, max_outer;              /* ICP iterations (100); ADMM iterations per ICP iteration (100) */
+  double stop;                         /* stopping threshold (1e-5, normalised units) */
+} flb_sicp_config;
+typedef struct flb_sicp_result {
+  double res_trans[16];                /* Registeration::run's res_trans, row-major 4x4, translation in the caller's units */
+  int status;                          /* FLB_FRICP_OK / _FEW_TARGET / _NO_SOURCE */
+  int iterations, admm_iterations;     /* ICP iterations; ADMM iterations over all of them */
+  double scale, mu_source[3], mu_target[3];   /* the normalisation: p_n = p / scale - mu */
+  int n_source, n_target;              /* source points; assembled target points */
+  int n_source_finite, n_target_finite;
+  double primal, dual, stop, mu_exit;  /* the last ICP iteration's max |P|, Σ|ΔX|²/n, max |X - X_prev| and μ at its exit */
+  int syncs;                           /* host synchronisations the call made */
+  int admm_blocks;                     /* blocks of 256 threads the ADMM kernel ran on (all resident) */
+  int log_n;                           /* rows written to out_log */
+} flb_sicp_result;
+/* Registeration's SICP::Parameters: p 0.4, mu 10, alpha 1.2, max_mu 1e5, max_icp 100, max_outer 100, stop 1e-5. */
+void flb_sicp_default_config(flb_sicp_config* cfg);
+/* Registers the source onto the target.  out_corr_index / out_resid (optional, n_src entries each) receive the last ICP
+ * iteration's matched target index and the residual |X - Q| of that match in normalised units, before its ADMM loop (-1
+ * and +inf for a non-finite source point or when nothing was matched).  out_log (optional, log_cap rows of 5 doubles): per
+ * ICP iteration the ADMM iterations, primal, dual, stop and μ at its exit. */
+int flb_keyframes_sicp(flb_keyframes* kf, const void* src_points, int n_src, int src_stride, int src_off_intensity,
+                       const float* src_pose6, const int* tgt_ids, int n_tgt, const float* tgt_pre_pose6, const float* tgt_poses6,
+                       const flb_sicp_config* cfg, flb_sicp_result* out, int* out_corr_index, double* out_resid,
+                       double* out_log, int log_cap);
+
 /* Stream access for callers that overlap work (returns a cudaStream_t as void*). */
 void* flb_session_stream(flb_session* s);
 int flb_session_sync(flb_session* s);
