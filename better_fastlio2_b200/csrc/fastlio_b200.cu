@@ -14,6 +14,7 @@
 #include <algorithm>
 #include <chrono>
 #include <climits>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -609,6 +610,16 @@ static int launch_knn(flb_map* m, KnnArgs a) {
 
 static int ensure_outbuf(flb_map* m, int n) { return grow(m->outbuf, sizeof(float4) * (size_t)n, sizeof(float4) << 16); }
 
+// The reference accepts a neighbour when its float distance satisfies dist <= max_dist * max_dist evaluated in double
+// (ikd_Tree.cpp:872,887).  For a float d2 that is the same as d2 <= the largest float not above the double square;
+// fl(max_dist * max_dist) is that float when it rounds down, but when it rounds up (0.1f) it admits a neighbour at
+// d2 = fl(max_dist * max_dist) that the reference rejects.
+static float max_d2_of(float max_dist) {
+  const double sq = (double)max_dist * (double)max_dist;
+  const float f = (float)sq;
+  return (double)f > sq ? std::nextafter(f, 0.f) : f;
+}
+
 static int nearest_search_impl(flb_map* m, const float* q_xyz, int nq, int stride, int k, float max_dist, float* out_pts, int out_w,
                                float* out_d2, int* out_cnt) {
   if (!m) return set_err("null map");
@@ -623,7 +634,7 @@ static int nearest_search_impl(flb_map* m, const float* q_xyz, int nq, int strid
   CU(cudaMalloc((void**)&dcnt, nq));
   KnnArgs a;
   a.m = m->d; a.q = m->stage.p; a.n = nq; a.nbr = m->outbuf.p; a.cnt = dcnt;
-  a.max_d2 = (max_dist > 0.f && max_dist < 1e18f) ? max_dist * max_dist : INFINITY;
+  a.max_d2 = (max_dist > 0.f && max_dist < 1e18f) ? max_d2_of(max_dist) : INFINITY;
   a.phase_stats = nullptr;
   a.ctl = nullptr; a.body = nullptr; a.stride = nq; a.work_count = nullptr;
   int lrc = (K == 5) ? launch_knn<5>(m, a) : launch_knn<20>(m, a);
@@ -636,7 +647,7 @@ static int nearest_search_impl(flb_map* m, const float* q_xyz, int nq, int strid
     hi.resize((size_t)nq * K);
     le = cudaMalloc((void**)&dint, sizeof(float) * hi.size());
     if (le == cudaSuccess) {
-      k_lookup_intensity<<<grid_for(nq * K, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->d, m->outbuf.p, dint, nq * K);
+      k_lookup_intensity<<<grid_for(nq * K, 256, m->sm_count * 8), 256, 0, m->stream>>>(m->d, m->outbuf.p, dint, nq, K);
       m->launches++;
       le = cudaMemcpyAsync(hi.data(), dint, sizeof(float) * hi.size(), cudaMemcpyDeviceToHost, m->stream);
     }

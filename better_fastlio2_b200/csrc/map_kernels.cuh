@@ -609,11 +609,19 @@ __global__ void k_coarse_rebuild(MapDev m, int nblk) {
 }
 
 // intensity of returned neighbours (API searches only; off the hot path): the neighbour's voxel is re-read and the point with
-// exactly these coordinates looked up.  pts: (x, y, z, d2) records, NaN x = no neighbour.
-__global__ void k_lookup_intensity(MapDev m, const float4* __restrict__ pts, float* __restrict__ out, int n) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+// exactly these coordinates looked up.  pts: [K][nq] (x, y, z, d2) records, NaN x = no neighbour.  A verbatim insert keeps
+// duplicate points, each with its own intensity: the r-th neighbour of a query takes the j-th coordinate match of its
+// chain, j = the number of that query's earlier neighbours with the same coordinates, so that every duplicate returned
+// carries a different record's intensity, as the reference returns each record.
+__global__ void k_lookup_intensity(MapDev m, const float4* __restrict__ pts, float* __restrict__ out, int nq, int K) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nq * K; i += gridDim.x * blockDim.x) {
     const float4 p = pts[i];
     float r = 0.f;
+    int skip = 0;
+    for (int e = i - nq; e >= 0; e -= nq) {
+      const float4 o = pts[e];
+      skip += (o.x == p.x && o.y == p.y && o.z == p.z) ? 1 : 0;
+    }
     if (p.x == p.x && coord_ok(p.x, p.y, p.z, m.ds)) {
       const int vx = voxel_of(p.x, m.ds), vy = voxel_of(p.y, m.ds), vz = voxel_of(p.z, m.ds);
       const int blk = find_block(m, pack_key(vx >> 2, vy >> 2, vz >> 2));
@@ -622,7 +630,7 @@ __global__ void k_lookup_intensity(MapDev m, const float4* __restrict__ pts, flo
         float4 e = m.slots[idx];
         float inten = m.sint[idx];
         for (;;) {
-          if (e.x == p.x && e.y == p.y && e.z == p.z) { r = inten; break; }
+          if (e.x == p.x && e.y == p.y && e.z == p.z && skip-- == 0) { r = inten; break; }
           const int c = __float_as_int(e.w);
           if (c < 0) break;
           e = m.ovf[c];

@@ -88,7 +88,8 @@ int flb_map_delete_boxes(flb_map* m, const float* boxes6, int nb, int* n_deleted
 int flb_map_delete_points(flb_map* m, const float* xyz, int n, int stride_bytes, int* n_deleted);
 /* Nearest_Search (ikd_Tree.cpp:366-397), batched over nq queries: exact k-NN (k <= 5 on the fast path, <= 20
  * otherwise) among valid points with float squared distances, ascending; max_dist <= 0 means unbounded (the
- * reference default INFINITY).  out_xyz[nq*k*3], out_d2[nq*k] (unfilled = NaN / INF), out_cnt[nq]. */
+ * reference default INFINITY), otherwise a neighbour is kept when d2 <= max_dist * max_dist in double, as the
+ * reference compares.  out_xyz[nq*k*3], out_d2[nq*k] (unfilled = NaN / INF), out_cnt[nq]. */
 int flb_map_nearest_search(flb_map* m, const float* q_xyz, int nq, int stride_bytes, int k, float max_dist,
                            float* out_xyz, float* out_d2, int* out_cnt);
 /* Box_Search (ikd_Tree.cpp:399-404) / Radius_Search (:406-411): points in a half-open box / within radius.
