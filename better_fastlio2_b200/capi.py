@@ -105,6 +105,17 @@ class SicpResult(C.Structure):
                 ("log_n", C.c_int)]
 
 
+class AaicpConfig(C.Structure):
+    _fields_ = [("max_icp", C.c_int), ("stop", C.c_double), ("error_overflow_threshold", C.c_double)]
+
+
+class AaicpResult(C.Structure):
+    _fields_ = [("res_trans", C.c_double * 16), ("status", C.c_int), ("iterations", C.c_int), ("accepted", C.c_int),
+                ("resets", C.c_int), ("history", C.c_int), ("energy", C.c_double), ("scale", C.c_double),
+                ("mu_source", C.c_double * 3), ("mu_target", C.c_double * 3), ("n_source", C.c_int), ("n_target", C.c_int),
+                ("n_source_finite", C.c_int), ("n_target_finite", C.c_int), ("syncs", C.c_int), ("log_n", C.c_int)]
+
+
 class IcpResult(C.Structure):
     _fields_ = [("final_transformation", C.c_float * 16), ("converged", C.c_int), ("iterations", C.c_int), ("state", C.c_int),
                 ("n_source", C.c_int), ("n_target", C.c_int), ("n_correspondences", C.c_int), ("fitness_score", C.c_double)]
@@ -135,6 +146,7 @@ EXPORTS = [
     "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
     "flb_keyframes_scan_context", "flb_keyframes_scan_contexts", "flb_keyframes_icp",
     "flb_fricp_default_config", "flb_keyframes_fricp", "flb_sicp_default_config", "flb_keyframes_sicp",
+    "flb_aaicp_default_config", "flb_keyframes_aaicp",
     "flb_frontend_camera_config", "flb_frontend_camera_image", "flb_frontend_points_colorize", "flb_frontend_points_to_imu",
 ]
 
@@ -242,6 +254,10 @@ def lib():
         L.flb_sicp_default_config.restype = None
         L.flb_keyframes_sicp.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, fp, vp, C.c_int, fp, fp, C.POINTER(SicpConfig),
                                          C.POINTER(SicpResult), vp, dp, dp, C.c_int]
+        L.flb_aaicp_default_config.argtypes = [C.POINTER(AaicpConfig)]
+        L.flb_aaicp_default_config.restype = None
+        L.flb_keyframes_aaicp.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, fp, vp, C.c_int, fp, fp, C.POINTER(AaicpConfig),
+                                          C.POINTER(AaicpResult), vp, dp, dp, C.c_int]
         _lib = L
     return _lib
 
@@ -1001,6 +1017,46 @@ class KeyFrameStore:
                "n_source": r.n_source, "n_target": r.n_target, "n_source_finite": r.n_source_finite,
                "n_target_finite": r.n_target_finite, "primal": r.primal, "dual": r.dual, "stop": r.stop, "mu_exit": r.mu_exit,
                "syncs": r.syncs, "admm_blocks": r.admm_blocks}
+        out = (res,)
+        if correspondences:
+            out += (idx[:n].copy(), resid[:n].copy())
+        if log:
+            out += (lg[:r.log_n].copy(),)
+        return out if len(out) > 1 else res
+
+    def aaicp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, max_icp=100, stop=1e-5,
+              error_overflow_threshold=0.05, correspondences=False, log=False, log_cap=4096):
+        """The relocaliser's AA-ICP (regMode 1) on the device, with the clouds of fricp(): the host source, moved by
+        src_pose6 when given, onto the key frames tgt_ids each moved by tgt_pre_pose6 when given and then by its tgt_poses6
+        row.  Returns a dict (res_trans (4,4) float64, status, status_name, iterations, accepted, resets, history, energy,
+        scale, mu_source, mu_target, n_source, n_target, n_source_finite, n_target_finite, syncs) and, in this order when
+        asked for, the last pass's matched target index (-1: none) and residual of every source point, and the
+        per-iteration log ((k, 6): energy, previous energy, outcome (-1 first, 1 accepted, 0 reset), α count,
+        |final - final_prev|_F, smallest alphas_cond margin)."""
+        pts, stride, off_i = self._source(src_points)
+        n = len(pts)
+        ids = np.ascontiguousarray(tgt_ids, np.int32).reshape(-1)
+        p6 = np.ascontiguousarray(tgt_poses6, np.float32).reshape(-1, 6)
+        if len(p6) != len(ids):
+            raise ValueError("one pose per target key frame")
+        pre = None if tgt_pre_pose6 is None else np.ascontiguousarray(tgt_pre_pose6, np.float32).reshape(6)
+        sp = None if src_pose6 is None else np.ascontiguousarray(src_pose6, np.float32).reshape(6)
+        cfg = AaicpConfig(int(max_icp), float(stop), float(error_overflow_threshold))
+        r = AaicpResult()
+        idx = resid = lg = None
+        if correspondences:
+            idx = np.empty(max(n, 1), np.int32)
+            resid = np.empty(max(n, 1), np.float64)
+        if log:
+            lg = np.zeros((max(int(log_cap), 1), 6), np.float64)
+        _chk(lib().flb_keyframes_aaicp(self.h, _p(pts) if n else None, n, stride, off_i, _p(sp), _p(ids) if len(ids) else None, len(ids),
+                                       _p(pre), _p(p6) if len(ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(resid), _p(lg),
+                                       int(log_cap) if log else 0))
+        res = {"res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
+               "status_name": FRICP_STATUS[r.status], "iterations": r.iterations, "accepted": r.accepted, "resets": r.resets,
+               "history": r.history, "energy": r.energy, "scale": r.scale, "mu_source": np.array(r.mu_source[:]),
+               "mu_target": np.array(r.mu_target[:]), "n_source": r.n_source, "n_target": r.n_target,
+               "n_source_finite": r.n_source_finite, "n_target_finite": r.n_target_finite, "syncs": r.syncs}
         out = (res,)
         if correspondences:
             out += (idx[:n].copy(), resid[:n].copy())

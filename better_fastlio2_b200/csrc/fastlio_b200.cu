@@ -1775,4 +1775,5 @@ extern "C" int flb_debug_trace_read(unsigned long long* out, long long* phases, 
 #include "icp_host.cuh"
 #include "fricp_host.cuh"
 #include "sicp_host.cuh"
+#include "aaicp_host.cuh"
 #include "color_host.cuh"

@@ -569,6 +569,48 @@ int flb_keyframes_sicp(flb_keyframes* kf, const void* src_points, int n_src, int
                        const flb_sicp_config* cfg, flb_sicp_result* out, int* out_corr_index, double* out_resid,
                        double* out_log, int log_cap);
 
+/* ------------------------------------------------------------------------------------------------ relocalisation AA-ICP
+ * The relocaliser's regMode 1 (AA-ICP, AAICP::point_to_point_aaicp, include/FRICP-toolkit/ICP.h:841-1033, with
+ * Registeration's ICP::Parameters: no robust function, no initial transform).  Source, target, the dropping of non-finite
+ * points and the normalisation are flb_keyframes_fricp's.  Each iteration matches every moved source point X = final X0
+ * to its exact nearest target point Q (double d², equal d²: the lower target index), takes the unweighted Kabsch step on
+ * (X, Q) into T, and mixes the 6-vectors (eulerAngles(0, 1, 2), t) of the transforms by Anderson acceleration over the
+ * whole history, restarting it when the energy Σ|X - Q|² rises by more than error_overflow_threshold relative.  The loop
+ * ends after max_icp iterations or when |final - final_prev|_F < stop after the first.  DESIGN.md §9 states the contract
+ * and its deviations.  One synchronisation per iteration; the Euler, QR and Anderson work runs on the host.  Every
+ * argument is checked before any device work; the store and the map are not modified.  The scratch is
+ * flb_keyframes_fricp's map-side key-frame scratch.  Statuses are FLB_FRICP_*; FEW_TARGET means no finite target point. */
+typedef struct flb_aaicp_config {
+  int max_icp;                         /* ICP::Parameters::max_icp (100), >= 0 */
+  double stop;                         /* stop (1e-5, normalised units), finite and >= 0 */
+  double error_overflow_threshold;     /* error_overflow_threshold_ (0.05), finite: the relative energy rise that resets */
+} flb_aaicp_config;
+typedef struct flb_aaicp_result {
+  double res_trans[16];                /* Registeration::run's res_trans, row-major 4x4, translation in the caller's units */
+  int status;                          /* FLB_FRICP_OK / _FEW_TARGET / _NO_SOURCE */
+  int iterations;                      /* par.convergence_iter: the loop index at exit (passes run - 1 when the stop test
+                                          ended the loop, max_icp otherwise) */
+  int accepted, resets;                /* Anderson steps taken; times the first heuristic reset the history */
+  int history;                         /* columns of the Anderson history u at exit */
+  double energy;                       /* convergence_energy: Σ |final X0 - Q|² over the last pass's matches */
+  double scale, mu_source[3], mu_target[3];   /* the normalisation: p_n = p / scale - mu */
+  int n_source, n_target;              /* source points; assembled target points */
+  int n_source_finite, n_target_finite;
+  int syncs;                           /* host synchronisations the call made */
+  int log_n;                           /* rows written to out_log */
+} flb_aaicp_result;
+/* Registeration's ICP::Parameters as AA-ICP reads them: max_icp 100, stop 1e-5, error_overflow_threshold 0.05. */
+void flb_aaicp_default_config(flb_aaicp_config* cfg);
+/* Registers the source onto the target.  out_corr_index / out_resid (optional, n_src entries each) receive the last
+ * pass's matched target index and |X - Q| in normalised units (-1 and +inf for a non-finite source point or when no pass
+ * ran).  out_log (optional, log_cap rows of 6 doubles): per iteration the energy, the previous energy before the first
+ * heuristic's test, the outcome (-1 the first iteration, 1 Anderson step accepted, 0 reset), the number of α in u_next,
+ * |final - final_prev|_F and the smallest margin of the alphas_cond tests made (+inf when none was made). */
+int flb_keyframes_aaicp(flb_keyframes* kf, const void* src_points, int n_src, int src_stride, int src_off_intensity,
+                        const float* src_pose6, const int* tgt_ids, int n_tgt, const float* tgt_pre_pose6, const float* tgt_poses6,
+                        const flb_aaicp_config* cfg, flb_aaicp_result* out, int* out_corr_index, double* out_resid,
+                        double* out_log, int log_cap);
+
 /* Stream access for callers that overlap work (returns a cudaStream_t as void*). */
 void* flb_session_stream(flb_session* s);
 int flb_session_sync(flb_session* s);

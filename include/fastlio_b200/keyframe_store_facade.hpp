@@ -24,6 +24,8 @@
 //   keyframes.fricp(*cloudBuffer[idx], initPose, nearIds, pose_ext, *poses6D, fr, T);
 //   // regMode 7 (Sparse ICP, registeration.h:143-146) on the same clouds
 //   flb::SicpParams sp;  keyframes.sicp(*cloudBuffer[idx], initPose, nearIds, pose_ext, *poses6D, sp, T);
+//   // regMode 1 (AA-ICP, registeration.h:86-91) on the same clouds
+//   flb::AaicpParams ap;  keyframes.aaicp(*cloudBuffer[idx], initPose, nearIds, pose_ext, *poses6D, ap, T);
 //
 // Poses6D is anything with points[k].{x, y, z, roll, pitch, yaw} (pcl::PointCloud<PointTypePose>); an affine is
 // anything with operator()(row, col) (Eigen::Affine3f).  Clouds come back with x, y, z, intensity and curvature set
@@ -79,6 +81,13 @@ struct FricpParams {
 struct SicpParams {
   flb_sicp_config cfg{};
   SicpParams() { flb_sicp_default_config(&cfg); }
+};
+
+// Registeration's ICP::Parameters as regMode 1 (AAICP::point_to_point_aaicp) reads them: max_icp, stop and
+// error_overflow_threshold_ (ICP.h:518-566).
+struct AaicpParams {
+  flb_aaicp_config cfg{};
+  AaicpParams() { flb_aaicp_default_config(&cfg); }
 };
 
 class KeyFrameStore {
@@ -241,6 +250,28 @@ class KeyFrameStore {
     if (!ok(flb_keyframes_sicp(kf_, p0, n, (int)sizeof(P), off_i, init6, ids.data(), (int)ids.size(), ext6, p6.data(), &params.cfg, &r,
                                nullptr, nullptr, nullptr, 0),
             "sicp"))
+      return false;
+    for (int i = 0; i < 4; ++i)
+      for (int j = 0; j < 4; ++j) T(i, j) = r.res_trans[4 * i + j];
+    if (info) *info = r;
+    return true;
+  }
+
+  // The same registration with regMode 1 (AA-ICP, registeration.h:86-91): the clouds of fricp(), the result into T.
+  template <class Cloud, class Pose, class Poses6D, class Mat>
+  bool aaicp(const Cloud& curCloud, const Pose& initPose, const std::vector<int>& ids, const Pose& pose_ext, const Poses6D& poses6D,
+             const AaicpParams& params, Mat& T, flb_aaicp_result* info = nullptr) {
+    typedef typename std::remove_reference<decltype(curCloud.points[0])>::type P;
+    const int n = (int)curCloud.points.size();
+    const P* p0 = n ? &curCloud.points[0] : nullptr;
+    const int off_i = n ? (int)((const char*)&p0->intensity - (const char*)p0) : -1;
+    const float init6[6] = {initPose.x, initPose.y, initPose.z, initPose.roll, initPose.pitch, initPose.yaw};
+    const float ext6[6] = {pose_ext.x, pose_ext.y, pose_ext.z, pose_ext.roll, pose_ext.pitch, pose_ext.yaw};
+    const std::vector<float> p6 = poses6(ids, poses6D);
+    flb_aaicp_result r{};
+    if (!ok(flb_keyframes_aaicp(kf_, p0, n, (int)sizeof(P), off_i, init6, ids.data(), (int)ids.size(), ext6, p6.data(), &params.cfg, &r,
+                                nullptr, nullptr, nullptr, 0),
+            "aaicp"))
       return false;
     for (int i = 0; i < 4; ++i)
       for (int j = 0; j < 4; ++j) T(i, j) = r.res_trans[4 * i + j];
