@@ -121,6 +121,10 @@ class IcpResult(C.Structure):
                 ("n_source", C.c_int), ("n_target", C.c_int), ("n_correspondences", C.c_int), ("fitness_score", C.c_double)]
 
 
+class IcpBatchStats(C.Structure):
+    _fields_ = [("rounds", C.c_int), ("setup_syncs", C.c_int), ("iteration_syncs", C.c_int)]
+
+
 K_CLASSES = ["transform", "knn", "residual", "reduce", "classify", "insert", "delete"]
 
 _lib = None
@@ -145,6 +149,7 @@ EXPORTS = [
     "flb_keyframes_download", "flb_keyframes_info", "flb_keyframes_size", "flb_map_reconstruct_from_keyframes",
     "flb_keyframes_assemble", "flb_map_release_keyframe_scratch",
     "flb_keyframes_scan_context", "flb_keyframes_scan_contexts", "flb_keyframes_icp",
+    "flb_keyframes_icp_batch",
     "flb_fricp_default_config", "flb_keyframes_fricp", "flb_sicp_default_config", "flb_keyframes_sicp",
     "flb_aaicp_default_config", "flb_keyframes_aaicp",
     "flb_frontend_camera_config", "flb_frontend_camera_image", "flb_frontend_points_colorize", "flb_frontend_points_to_imu",
@@ -246,6 +251,8 @@ def lib():
         L.flb_keyframes_scan_contexts.argtypes = [vp, vp, C.c_int, C.c_double, dp]
         L.flb_keyframes_icp.argtypes = [vp, vp, C.c_int, C.c_int, fp, fp, vp, C.c_int, C.c_int, fp, C.POINTER(IcpConfig),
                                         C.POINTER(IcpResult), vp, fp]
+        L.flb_keyframes_icp_batch.argtypes = [vp, C.c_int, vp, vp, fp, vp, vp, fp, C.c_float, C.POINTER(IcpConfig),
+                                              C.POINTER(IcpResult), C.POINTER(IcpBatchStats)]
         L.flb_fricp_default_config.argtypes = [C.POINTER(FricpConfig)]
         L.flb_fricp_default_config.restype = None
         L.flb_keyframes_fricp.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, fp, vp, C.c_int, fp, fp, C.POINTER(FricpConfig),
@@ -930,6 +937,41 @@ class KeyFrameStore:
         if correspondences:
             return res, idx[:r.n_source].copy(), d2[:r.n_source].copy()
         return res
+
+    def icp_batch(self, pairs, leaf=0.2, max_correspondence_distance=30.0, max_iterations=10, transformation_epsilon=1e-6,
+                  euclidean_fitness_epsilon=1e-6):
+        """The multi-session mapper's inter-session registrations in one call: pairs is a list of (src_ids, src_poses6,
+        tgt_ids, tgt_poses6), each selection assembled with its key frames' poses6 and, for leaf > 0, VoxelGrid-filtered
+        (as assemble(ids, poses6, leaf=leaf)), then registered as icp() registers it.  Returns (a list of icp()'s dicts,
+        one per pair, with n_source / n_target the filtered sizes, and a dict of rounds, setup_syncs, iteration_syncs)."""
+        sides = ([], [], [], [])
+        for src_ids, src_p6, tgt_ids, tgt_p6 in pairs:
+            for j, (ids, p6) in enumerate(((src_ids, src_p6), (tgt_ids, tgt_p6))):
+                ids = np.ascontiguousarray(ids, np.int32).reshape(-1)
+                p6 = np.ascontiguousarray(p6, np.float32).reshape(-1)
+                if len(p6) != 6 * len(ids):
+                    raise ValueError("one pose6 per selected key frame")
+                sides[2 * j].append(ids)
+                sides[2 * j + 1].append(p6)
+        n = len(pairs)
+        offs = [np.zeros(n + 1, np.int32), np.zeros(n + 1, np.int32)]
+        cat = []
+        for j in range(2):
+            offs[j][1:] = np.cumsum([len(a) for a in sides[2 * j]]) if n else []
+            cat.append(np.concatenate(sides[2 * j]) if n else np.zeros(0, np.int32))
+            cat.append(np.concatenate(sides[2 * j + 1]) if n else np.zeros(0, np.float32))
+        cfg = IcpConfig(float(max_correspondence_distance), int(max_iterations), float(transformation_epsilon),
+                        float(euclidean_fitness_epsilon))
+        res = (IcpResult * max(n, 1))()
+        st = IcpBatchStats()
+        _chk(lib().flb_keyframes_icp_batch(self.h, n, _p(offs[0]), _p(cat[0]) if len(cat[0]) else None,
+                                           _p(cat[1]) if len(cat[0]) else None, _p(offs[1]), _p(cat[2]) if len(cat[2]) else None,
+                                           _p(cat[3]) if len(cat[2]) else None, float(leaf), C.byref(cfg), res, C.byref(st)))
+        out = [{"final_transformation": np.array(r.final_transformation[:], np.float32).reshape(4, 4), "converged": bool(r.converged),
+                "iterations": r.iterations, "state": r.state, "state_name": ICP_STATES[r.state], "n_source": r.n_source,
+                "n_target": r.n_target, "n_correspondences": r.n_correspondences, "fitness_score": r.fitness_score}
+               for r in res[:n]]
+        return out, {"rounds": st.rounds, "setup_syncs": st.setup_syncs, "iteration_syncs": st.iteration_syncs}
 
     def fricp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, mode=4, max_icp=100, stop=1e-5,
               anderson_m=5, nu_begin_k=3.0, nu_end_k=1.0 / (3.0 * np.sqrt(3.0)), nu_alpha=0.5, correspondences=False, log=False,

@@ -1773,6 +1773,7 @@ extern "C" int flb_debug_trace_read(unsigned long long* out, long long* phases, 
 #include "keyframe_host.cuh"
 #include "scan_context_host.cuh"
 #include "icp_host.cuh"
+#include "icp_batch_host.cuh"
 #include "fricp_host.cuh"
 #include "sicp_host.cuh"
 #include "aaicp_host.cuh"

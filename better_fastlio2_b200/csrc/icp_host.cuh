@@ -92,35 +92,43 @@ static int icp_bounds(flb_map* m, IcpIndex& x, const float4* p, int n, float* lo
   return 0;
 }
 
-// The grid index over the target t[0, n): *n_fin finite points (0: nothing more is built), the grid *g over their box,
-// the finite points sorted by cell into x.sorted (their original indices in x.vals_b), CSR offsets and coarse boxes.
+// The grid index over the target t[0, n) on grid g, whose box holds its n_fin finite points: the finite points sorted by
+// cell into sorted (w = the original index; x.vals_b the sorted original indices), the CSR offsets cs and the coarse boxes
+// box.
+static int icp_build(flb_map* m, IcpIndex& x, const float4* t, int n, const IcpGrid& g, int n_fin, float4* sorted, int* cs, IcpBox* box) {
+  const unsigned n_cells = (unsigned)g.gx * g.gy * g.gz;
+  const int n_coarse = g.cx * g.cy * g.cz;
+  size_t tb = x.tmp.cap;
+  k_icp_keys<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(g, t, n, x.keys_a.p, x.vals_a.p);
+  CU(cub::DeviceRadixSort::SortPairs(x.tmp.p, tb, (const unsigned*)x.keys_a.p, x.keys_b.p, (const int*)x.vals_a.p, x.vals_b.p, n, 0, 32,
+                                     m->stream));
+  k_icp_gather<<<grid_for(n_fin, 256, m->sm_count * 8), 256, 0, m->stream>>>(x.vals_b.p, t, n_fin, sorted);
+  k_icp_cell_start<<<grid_for(n_fin + 1, 256, m->sm_count * 8), 256, 0, m->stream>>>(x.keys_b.p, n_fin, n_cells, cs);
+  k_icp_coarse_boxes<<<grid_for(n_coarse, 8, m->sm_count * 8), 256, 0, m->stream>>>(sorted, cs, n_coarse, box);
+  m->launches += 4 + 5;   // + the radix sort's kernels
+  CU(cudaGetLastError());
+  return 0;
+}
+
+// The grid index over the target t[0, n) into x: *n_fin finite points (0: nothing more is built), the grid *g over their
+// box, then icp_build into x.sorted, x.cs and x.box.
 static int icp_index(flb_map* m, IcpIndex& x, const float4* t, int n, IcpGrid* g, int* n_fin) {
   float lo[3], hi[3];
   if (icp_bounds(m, x, t, n, lo, hi, n_fin)) return 1;
   const int nf = *n_fin;
   if (nf == 0) return 0;
   *g = icp_grid(lo, hi, nf);
-  const unsigned n_cells = (unsigned)g->gx * g->gy * g->gz;
-  const int n_coarse = g->cx * g->cy * g->cz;
-  if (grow(x.cs, sizeof(int) * ((size_t)n_cells + 1), 0) || grow(x.box, sizeof(IcpBox) * (size_t)n_coarse, 0)) return 1;
-  size_t tb = x.tmp.cap;
-  k_icp_keys<<<grid_for(n, 256, m->sm_count * 8), 256, 0, m->stream>>>(*g, t, n, x.keys_a.p, x.vals_a.p);
-  CU(cub::DeviceRadixSort::SortPairs(x.tmp.p, tb, (const unsigned*)x.keys_a.p, x.keys_b.p, (const int*)x.vals_a.p, x.vals_b.p, n, 0, 32,
-                                     m->stream));
-  k_icp_gather<<<grid_for(nf, 256, m->sm_count * 8), 256, 0, m->stream>>>(x.vals_b.p, t, nf, x.sorted.p);
-  k_icp_cell_start<<<grid_for(nf + 1, 256, m->sm_count * 8), 256, 0, m->stream>>>(x.keys_b.p, nf, n_cells, x.cs.p);
-  k_icp_coarse_boxes<<<grid_for(n_coarse, 8, m->sm_count * 8), 256, 0, m->stream>>>(x.sorted.p, x.cs.p, n_coarse, x.box.p);
-  m->launches += 4 + 5;   // + the radix sort's kernels
-  CU(cudaGetLastError());
-  return 0;
+  const size_t n_cells = (size_t)g->gx * g->gy * g->gz, n_coarse = (size_t)g->cx * g->cy * g->cz;
+  if (grow(x.cs, sizeof(int) * (n_cells + 1), 0) || grow(x.box, sizeof(IcpBox) * n_coarse, 0)) return 1;
+  return icp_build(m, x, t, n, *g, nf, x.sorted.p, x.cs.p, x.box.p);
 }
 
 // The queries' visiting order: the keys the caller's key kernel wrote to x.keys_a (x.vals_a the identity), sorted into
-// x.order.
-static int icp_order(flb_map* m, IcpIndex& x, int n_s) {
+// order (x.order unless given).
+static int icp_order(flb_map* m, IcpIndex& x, int n_s, int* order = nullptr) {
   size_t tb = x.tmp.cap;
-  CU(cub::DeviceRadixSort::SortPairs(x.tmp.p, tb, (const unsigned*)x.keys_a.p, x.keys_b.p, (const int*)x.vals_a.p, x.order.p, n_s, 0, 32,
-                                     m->stream));
+  CU(cub::DeviceRadixSort::SortPairs(x.tmp.p, tb, (const unsigned*)x.keys_a.p, x.keys_b.p, (const int*)x.vals_a.p, order ? order : x.order.p,
+                                     n_s, 0, 32, m->stream));
   m->launches += 5;   // the radix sort's kernels
   CU(cudaGetLastError());
   return 0;

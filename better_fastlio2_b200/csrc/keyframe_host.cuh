@@ -4,6 +4,7 @@
 // (saveMapService :1763-1798, the per-key-frame saver :2501-2530).  Every reader assembles its selection with one
 // k_kf_assemble launch.  Included at the end of fastlio_b200.cu after frontend_host.cuh (uses VgWork, flb_frontend).
 #pragma once
+#include "icp_batch_kernels.cuh"
 #include "icp_kernels.cuh"
 #include "keyframe_kernels.cuh"
 #include "scan_context_kernels.cuh"
@@ -35,6 +36,21 @@ struct IcpWork {
   DevBuf<float> corr_d2;
   DevBuf<double> sums;                         // the pairs record (8) and the cross products (9)
   PinnedBuf<double> h_sums;
+};
+
+// flb_keyframes_icp_batch's own scratch (icp_batch_host.cuh): one round's pairs packed back to back
+struct IcpBatchWork {
+  DevBuf<float4> raw;                          // dense assembly of one selection before its voxel grid
+  DevBuf<float4> src, tgt, x, sorted;          // sources, targets, moved sources, sorted finite targets (w = index)
+  DevBuf<int> order, corr, cs;                 // sources' visiting order, nearest target per source, CSR cell offsets
+  DevBuf<float> corr_d2;
+  DevBuf<int2> open;                           // open queries of the fine rings (source index, item)
+  DevBuf<IcpBox> box;                          // coarse-cell point boxes
+  DevBuf<IcpBatchItem> items;                  // the active pairs of a pass
+  PinnedBuf<IcpBatchItem> h_items;             //   and their staging
+  DevBuf<double> partials, sums;               // reduction block partials; the pairs' sum records (ICPB_REC each)
+  PinnedBuf<double> h_sums;
+  DevBuf<unsigned> counters;                   // one reduction counter per pair, then the open count
 };
 
 // flb_keyframes_fricp's own scratch (fricp_host.cuh)
@@ -70,6 +86,7 @@ struct KfWork {
   PinnedBuf<unsigned> h_sc_keys;               //   and their staging
   IcpIndex index;                              // the registrations' target index and reductions
   IcpWork icp;                                 // flb_keyframes_icp's sub-maps and matches
+  IcpBatchWork icpb;                           // flb_keyframes_icp_batch's packed rounds
   FricpWork fricp;                             // flb_keyframes_fricp's clouds, matches and medians
   SicpWork sicp;                               // flb_keyframes_sicp's ADMM state
 };
@@ -120,6 +137,9 @@ static long long kf_scratch_bytes(const flb_map* m) {
     b += x.sorted.cap + x.keys_a.cap + x.keys_b.cap + x.vals_a.cap + x.vals_b.cap + x.order.cap + x.open.cap + x.cs.cap + x.box.cap +
          x.tmp.cap + x.partials.cap + x.misc.cap;
     b += i.src_raw.cap + i.src.cap + i.x.cap + i.tgt.cap + i.corr.cap + i.corr_d2.cap + i.sums.cap;
+    const IcpBatchWork& bw = w->icpb;
+    b += bw.raw.cap + bw.src.cap + bw.tgt.cap + bw.x.cap + bw.sorted.cap + bw.order.cap + bw.corr.cap + bw.cs.cap + bw.corr_d2.cap +
+         bw.open.cap + bw.box.cap + bw.items.cap + bw.partials.cap + bw.sums.cap + bw.counters.cap;
     b += f.raw.cap + f.src_raw.cap + f.src.cap + f.tgt_a.cap + f.tgt.cap + f.tgtf.cap + f.x.cap + f.tn.cap + f.sorted_d.cap + f.pos.cap +
          f.corr.cap + f.d2.cap + f.med.cap + f.sort_a.cap + f.sort_b.cap + f.sums.cap;
     const SicpWork& s = w->sicp;

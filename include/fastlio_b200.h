@@ -477,6 +477,35 @@ int flb_keyframes_icp(flb_keyframes* kf, const int* src_ids, int n_src, int src_
                       const float* src_pre_pose6, const int* tgt_ids, int n_tgt, int tgt_kind, const float* tgt_transforms,
                       const flb_icp_config* cfg, flb_icp_result* out, int* out_corr_index, float* out_corr_d2);
 
+/* ------------------------------------------------------------------------------------------------ inter-session registration
+ * IncreMapping::run's inter-session loops (multi-session Incremental_mapping.cpp: addSCloops :651-696 with
+ * doICPVirtualRelative :462-522, addRSloops :787-837 with doICPGlobalRelative :525-583), every pair of a round in one
+ * call.  Pair p's source is src_ids[src_offsets[p] .. src_offsets[p+1]), each key frame moved by its own src_poses6 row
+ * (FLB_KF_POSE6: transformPointCloud(.., &PointTypePose), a zero pose computed, not copied, as
+ * loopFindNearKeyframesLocalCoord :119-139 does), concatenated as flb_keyframes_assemble writes it and, for
+ * leaf_size > 0, VoxelGrid-filtered exactly as that call filters (PCL's int32 overflow guard included); leaf_size == 0
+ * keeps the dense concatenation.  The target is built the same way from tgt_offsets / tgt_ids / tgt_poses6.  Each pair is
+ * then registered as flb_keyframes_icp registers it (identity guess, no pre-pose): out[p] is that call's result on the
+ * same clouds, bit for bit, with n_source / n_target the sizes after filtering.  An empty source, or a target without a
+ * finite point, gives flb_keyframes_icp's empty result.  The pairs run in lockstep: each iteration is one exact 1-NN pass
+ * over every active pair, one copy and one synchronisation; a pair that stops (converged or NO_CORRESPONDENCES) leaves
+ * the lockstep and the others go on.  Pairs are packed in order into rounds whose summed grid cells stay within 2^27 (at
+ * least one pair per round); a pair's result depends only on its own selections, never on its round or the other pairs.
+ * Every argument is checked before any device work and an error names the pair and the field; n_pairs == 0 does
+ * nothing.  The store and the map are not modified; the packed clouds and indices are map-side key-frame scratch
+ * (flb_keyframes_info, flb_map_release_keyframe_scratch).  DESIGN.md §9 "Inter-session registration". */
+typedef struct flb_icp_batch_stats {
+  int rounds;            /* rounds the call split the batch into (pairs registered together in lockstep) */
+  int setup_syncs;       /* host synchronisations spent on assembly, filters and index builds (one per filtered
+                            selection, one per target box) */
+  int iteration_syncs;   /* host synchronisations of the lockstep iterations and the fitness passes: per round, the most
+                            passes any of its pairs ran (its iterations, plus one if it stopped with NO_CORRESPONDENCES),
+                            plus one for the fitness pass */
+} flb_icp_batch_stats;
+int flb_keyframes_icp_batch(flb_keyframes* kf, int n_pairs, const int* src_offsets, const int* src_ids, const float* src_poses6,
+                            const int* tgt_offsets, const int* tgt_ids, const float* tgt_poses6, float leaf_size,
+                            const flb_icp_config* cfg, flb_icp_result* out /* n_pairs */, flb_icp_batch_stats* stats /* may be NULL */);
+
 /* ------------------------------------------------------------------------------------------------ relocalisation registration
  * The online relocaliser's registration (pose_estimator::run, reg[0].run(curCloud, nearCloud), pose_estimator.cpp:180-269,
  * :566-596): FRICP<3>::point_to_point as Registeration::run (include/FRICP-toolkit/registeration.h:36-175) calls it, for

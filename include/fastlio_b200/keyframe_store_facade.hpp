@@ -19,6 +19,10 @@
 //   // the ICP of performLoopClosure (:946-974) once the gate passed: the same selections, com = the SC yaw pose
 //   flb::IcpParams icp;  icp.setMaxCorrespondenceDistance(200); ...;  flb::IcpResult reg;
 //   keyframes.icp(curIds, curT, com, preIds, preT, icp, reg);  reg.hasConverged(), reg.getFitnessScore(), ...
+//   // the multi-session mapper's inter-session loops (Incremental_mapping.cpp addSCloops :651-696, addRSloops :787-837):
+//   // both sessions' key frames in one store, one IcpPairSel per loop pair, every pair of the loop list in one call
+//   flb::IcpPairSel sel;  sel.addSrc(id, pose);  sel.addTgt(id, pose);  ...;  std::vector<flb::IcpResult> regs;
+//   keyframes.icp_batch(pairs, 0.2f, icp, regs);  regs[p].hasConverged(), regs[p].getFitnessScore(), ...
 //   // the relocaliser (pose_estimator.cpp:184-198, :566-596), the prior session's key frames pushed back once:
 //   flb::FricpParams fr(regMode);  Eigen::MatrixXd T(4, 4);
 //   keyframes.fricp(*cloudBuffer[idx], initPose, nearIds, pose_ext, *poses6D, fr, T);
@@ -64,6 +68,22 @@ struct IcpResult {
   void getFinalTransformation(M& T) const {
     for (int i = 0; i < 4; ++i)
       for (int j = 0; j < 4; ++j) T(i, j) = r.final_transformation[4 * i + j];
+  }
+};
+
+// One pair of flb_keyframes_icp_batch: the source and the target selections, each key frame with its own pose (anything
+// with x, y, z, roll, pitch, yaw: PointTypePose; a zero pose for the local-frame Scan Context pairs).
+struct IcpPairSel {
+  std::vector<int> srcIds, tgtIds;
+  std::vector<float> srcPoses6, tgtPoses6;   // 6 per id
+  template <class Pose> void addSrc(int id, const Pose& p) { add(srcIds, srcPoses6, id, p); }
+  template <class Pose> void addTgt(int id, const Pose& p) { add(tgtIds, tgtPoses6, id, p); }
+
+ private:
+  template <class Pose>
+  static void add(std::vector<int>& ids, std::vector<float>& p6, int id, const Pose& p) {
+    ids.push_back(id);
+    p6.insert(p6.end(), {p.x, p.y, p.z, p.roll, p.pitch, p.yaw});
   }
 };
 
@@ -207,6 +227,37 @@ class KeyFrameStore {
     return ok(flb_keyframes_icp(kf_, curIds.data(), (int)curIds.size(), FLB_KF_AFFINE, a.data(), pre, preIds.data(), (int)preIds.size(),
                                 FLB_KF_AFFINE, b.data(), &params.cfg, &result.r, nullptr, nullptr),
               "icp");
+  }
+
+  // IncreMapping's inter-session registrations (doICPVirtualRelative :462-522, doICPGlobalRelative :525-583) of every
+  // pair in one call: each selection assembled with its poses and VoxelGrid(leaf)-filtered (leaf 0: dense), each pair
+  // registered as icp() registers it with no pre-pose.  results[p] is pair p's registration; stats may be null.
+  bool icp_batch(const std::vector<IcpPairSel>& pairs, float leaf, const IcpParams& params, std::vector<IcpResult>& results,
+                 flb_icp_batch_stats* stats = nullptr) {
+    results.assign(pairs.size(), IcpResult());
+    if (params.ransac_iterations != 0) {
+      std::fprintf(stderr, "[fastlio_b200] KeyFrameStore::icp_batch: RANSAC rejection is not offered (setRANSACIterations(0))\n");
+      return false;
+    }
+    std::vector<int> so(1, 0), to(1, 0), si, ti;
+    std::vector<float> sp, tp;
+    for (const IcpPairSel& q : pairs) {
+      if (q.srcPoses6.size() != 6 * q.srcIds.size() || q.tgtPoses6.size() != 6 * q.tgtIds.size())
+        return ok(1, "icp_batch: one pose per key frame");
+      si.insert(si.end(), q.srcIds.begin(), q.srcIds.end());
+      ti.insert(ti.end(), q.tgtIds.begin(), q.tgtIds.end());
+      sp.insert(sp.end(), q.srcPoses6.begin(), q.srcPoses6.end());
+      tp.insert(tp.end(), q.tgtPoses6.begin(), q.tgtPoses6.end());
+      so.push_back((int)si.size());
+      to.push_back((int)ti.size());
+    }
+    std::vector<flb_icp_result> r(pairs.size() + 1);
+    if (!ok(flb_keyframes_icp_batch(kf_, (int)pairs.size(), so.data(), si.data(), sp.data(), to.data(), ti.data(), tp.data(), leaf,
+                                    &params.cfg, r.data(), stats),
+            "icp_batch"))
+      return false;
+    for (size_t p = 0; p < pairs.size(); ++p) results[p].r = r[p];
+    return true;
   }
 
   // pose_estimator::run's registration (pose_estimator.cpp:184-198) with the prior session's key frames in the store:
