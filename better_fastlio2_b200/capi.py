@@ -908,6 +908,12 @@ class KeyFrameStore:
                                                _p(out) if len(ids) else None))
         return out
 
+    @staticmethod
+    def _icp_dict(r):
+        return {"final_transformation": np.array(r.final_transformation[:], np.float32).reshape(4, 4), "converged": bool(r.converged),
+                "iterations": r.iterations, "state": r.state, "state_name": ICP_STATES[r.state], "n_source": r.n_source,
+                "n_target": r.n_target, "n_correspondences": r.n_correspondences, "fitness_score": r.fitness_score}
+
     def icp(self, src_ids, tgt_ids, src_poses6=None, src_affines=None, tgt_poses6=None, tgt_affines=None, pre_pose6=None,
             max_correspondence_distance=200.0, max_iterations=100, transformation_epsilon=1e-6, euclidean_fitness_epsilon=1e-6,
             correspondences=False):
@@ -931,9 +937,7 @@ class KeyFrameStore:
         _chk(lib().flb_keyframes_icp(self.h, _p(src_ids) if len(src_ids) else None, len(src_ids), sk, _p(st) if len(src_ids) else None,
                                      _p(pre), _p(tgt_ids) if len(tgt_ids) else None, len(tgt_ids), tk,
                                      _p(tt) if len(tgt_ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(d2)))
-        res = {"final_transformation": np.array(r.final_transformation[:], np.float32).reshape(4, 4), "converged": bool(r.converged),
-               "iterations": r.iterations, "state": r.state, "state_name": ICP_STATES[r.state], "n_source": r.n_source,
-               "n_target": r.n_target, "n_correspondences": r.n_correspondences, "fitness_score": r.fitness_score}
+        res = self._icp_dict(r)
         if correspondences:
             return res, idx[:r.n_source].copy(), d2[:r.n_source].copy()
         return res
@@ -967,11 +971,8 @@ class KeyFrameStore:
         _chk(lib().flb_keyframes_icp_batch(self.h, n, _p(offs[0]), _p(cat[0]) if len(cat[0]) else None,
                                            _p(cat[1]) if len(cat[0]) else None, _p(offs[1]), _p(cat[2]) if len(cat[2]) else None,
                                            _p(cat[3]) if len(cat[2]) else None, float(leaf), C.byref(cfg), res, C.byref(st)))
-        out = [{"final_transformation": np.array(r.final_transformation[:], np.float32).reshape(4, 4), "converged": bool(r.converged),
-                "iterations": r.iterations, "state": r.state, "state_name": ICP_STATES[r.state], "n_source": r.n_source,
-                "n_target": r.n_target, "n_correspondences": r.n_correspondences, "fitness_score": r.fitness_score}
-               for r in res[:n]]
-        return out, {"rounds": st.rounds, "setup_syncs": st.setup_syncs, "iteration_syncs": st.iteration_syncs}
+        stats = {"rounds": st.rounds, "setup_syncs": st.setup_syncs, "iteration_syncs": st.iteration_syncs}
+        return [self._icp_dict(r) for r in res[:n]], stats
 
     def fricp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, mode=4, max_icp=100, stop=1e-5,
               anderson_m=5, nu_begin_k=3.0, nu_end_k=1.0 / (3.0 * np.sqrt(3.0)), nu_alpha=0.5, correspondences=False, log=False,
@@ -983,40 +984,16 @@ class KeyFrameStore:
         mu_target, nu_begin, nu_end, energy, n_source, n_target, n_source_finite, n_target_finite) and, in this order when
         asked for, the last pass's matched target index (-1: none) and residual of every source point, and the
         per-iteration log ((k, 5): stage, energy, previous accepted energy, |T - T_prev|_F, accepted)."""
-        pts = np.ascontiguousarray(src_points, np.float32)
-        if pts.ndim != 2 or pts.shape[1] not in (3, 4, 12):
-            raise ValueError("src_points must be (n,3), (n,4) or (n,12) float32")
-        stride = 4 * pts.shape[1]
-        off_i = -1 if pts.shape[1] == 3 else (12 if pts.shape[1] == 4 else OFF_INTENSITY)
-        n = len(pts)
-        ids = np.ascontiguousarray(tgt_ids, np.int32).reshape(-1)
-        p6 = np.ascontiguousarray(tgt_poses6, np.float32).reshape(-1, 6)
-        if len(p6) != len(ids):
-            raise ValueError("one pose per target key frame")
-        pre = None if tgt_pre_pose6 is None else np.ascontiguousarray(tgt_pre_pose6, np.float32).reshape(6)
-        sp = None if src_pose6 is None else np.ascontiguousarray(src_pose6, np.float32).reshape(6)
-        cfg = FricpConfig(int(mode), int(max_icp), float(stop), int(anderson_m), float(nu_begin_k), float(nu_end_k), float(nu_alpha))
-        r = FricpResult()
-        idx = resid = lg = None
-        if correspondences:
-            idx = np.empty(max(n, 1), np.int32)
-            resid = np.empty(max(n, 1), np.float64)
-        if log:
-            lg = np.zeros((max(int(log_cap), 1), 5), np.float64)
-        _chk(lib().flb_keyframes_fricp(self.h, _p(pts) if n else None, n, stride, off_i, _p(sp), _p(ids) if len(ids) else None, len(ids),
-                                       _p(pre), _p(p6) if len(ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(resid), _p(lg),
-                                       int(log_cap) if log else 0))
-        res = {"res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
-               "status_name": FRICP_STATUS[r.status], "stages": r.stages, "iterations": r.iterations, "rejections": r.rejections,
-               "scale": r.scale, "mu_source": np.array(r.mu_source[:]), "mu_target": np.array(r.mu_target[:]),
-               "nu_begin": r.nu_begin, "nu_end": r.nu_end, "energy": r.energy, "n_source": r.n_source, "n_target": r.n_target,
-               "n_source_finite": r.n_source_finite, "n_target_finite": r.n_target_finite}
-        out = (res,)
-        if correspondences:
-            out += (idx[:n].copy(), resid[:n].copy())
-        if log:
-            out += (lg[:r.log_n].copy(),)
-        return out if len(out) > 1 else res
+        def cfg():
+            return FricpConfig(int(mode), int(max_icp), float(stop), int(anderson_m), float(nu_begin_k), float(nu_end_k),
+                               float(nu_alpha))
+        return self._reloc("flb_keyframes_fricp", cfg, FricpResult(), lambda r: {
+            "res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
+            "status_name": FRICP_STATUS[r.status], "stages": r.stages, "iterations": r.iterations, "rejections": r.rejections,
+            "scale": r.scale, "mu_source": np.array(r.mu_source[:]), "mu_target": np.array(r.mu_target[:]),
+            "nu_begin": r.nu_begin, "nu_end": r.nu_end, "energy": r.energy, "n_source": r.n_source, "n_target": r.n_target,
+            "n_source_finite": r.n_source_finite, "n_target_finite": r.n_target_finite},
+            src_points, tgt_ids, tgt_poses6, tgt_pre_pose6, src_pose6, correspondences, log, log_cap, 5)
 
     @staticmethod
     def _source(src_points):
@@ -1026,14 +1003,11 @@ class KeyFrameStore:
         off_i = -1 if pts.shape[1] == 3 else (12 if pts.shape[1] == 4 else OFF_INTENSITY)
         return pts, 4 * pts.shape[1], off_i
 
-    def sicp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, p=0.4, mu=10.0, alpha=1.2, max_mu=1e5,
-             max_icp=100, max_outer=100, stop=1e-5, correspondences=False, log=False, log_cap=4096):
-        """The relocaliser's Sparse ICP (regMode 7) on the device, with the clouds of fricp(): the host source, moved by
-        src_pose6 when given, onto the key frames tgt_ids each moved by tgt_pre_pose6 when given and then by its tgt_poses6
-        row.  Returns a dict (res_trans (4,4) float64, status, status_name, iterations, admm_iterations, scale, mu_source,
-        mu_target, n_source, n_target, n_source_finite, n_target_finite, primal, dual, stop, mu_exit, syncs, admm_blocks) and, in this
-        order when asked for, the last ICP iteration's matched target index (-1: none) and residual of every source point,
-        and the per-ICP-iteration log ((k, 5): ADMM iterations, primal, dual, stop, μ at exit)."""
+    def _reloc(self, fn, make_cfg, r, as_dict, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6, src_pose6, correspondences, log,
+               log_cap, log_width):
+        """fricp / sicp / aaicp through the C entry point named fn with the config make_cfg() (built once the clouds are
+        checked) into the result struct r: as_dict(r) and, in this order when asked for, the matched target index and
+        residual of every source point and the log (log_width columns)."""
         pts, stride, off_i = self._source(src_points)
         n = len(pts)
         ids = np.ascontiguousarray(tgt_ids, np.int32).reshape(-1)
@@ -1042,29 +1016,42 @@ class KeyFrameStore:
             raise ValueError("one pose per target key frame")
         pre = None if tgt_pre_pose6 is None else np.ascontiguousarray(tgt_pre_pose6, np.float32).reshape(6)
         sp = None if src_pose6 is None else np.ascontiguousarray(src_pose6, np.float32).reshape(6)
-        cfg = SicpConfig(float(p), float(mu), float(alpha), float(max_mu), int(max_icp), int(max_outer), float(stop))
-        r = SicpResult()
+        cfg = make_cfg()
         idx = resid = lg = None
         if correspondences:
             idx = np.empty(max(n, 1), np.int32)
             resid = np.empty(max(n, 1), np.float64)
         if log:
-            lg = np.zeros((max(int(log_cap), 1), 5), np.float64)
-        _chk(lib().flb_keyframes_sicp(self.h, _p(pts) if n else None, n, stride, off_i, _p(sp), _p(ids) if len(ids) else None, len(ids),
-                                      _p(pre), _p(p6) if len(ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(resid), _p(lg),
-                                      int(log_cap) if log else 0))
-        res = {"res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
-               "status_name": FRICP_STATUS[r.status], "iterations": r.iterations, "admm_iterations": r.admm_iterations,
-               "scale": r.scale, "mu_source": np.array(r.mu_source[:]), "mu_target": np.array(r.mu_target[:]),
-               "n_source": r.n_source, "n_target": r.n_target, "n_source_finite": r.n_source_finite,
-               "n_target_finite": r.n_target_finite, "primal": r.primal, "dual": r.dual, "stop": r.stop, "mu_exit": r.mu_exit,
-               "syncs": r.syncs, "admm_blocks": r.admm_blocks}
+            lg = np.zeros((max(int(log_cap), 1), log_width), np.float64)
+        _chk(getattr(lib(), fn)(self.h, _p(pts) if n else None, n, stride, off_i, _p(sp), _p(ids) if len(ids) else None, len(ids),
+                                _p(pre), _p(p6) if len(ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(resid), _p(lg),
+                                int(log_cap) if log else 0))
+        res = as_dict(r)
         out = (res,)
         if correspondences:
             out += (idx[:n].copy(), resid[:n].copy())
         if log:
             out += (lg[:r.log_n].copy(),)
         return out if len(out) > 1 else res
+
+    def sicp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, p=0.4, mu=10.0, alpha=1.2, max_mu=1e5,
+             max_icp=100, max_outer=100, stop=1e-5, correspondences=False, log=False, log_cap=4096):
+        """The relocaliser's Sparse ICP (regMode 7) on the device, with the clouds of fricp(): the host source, moved by
+        src_pose6 when given, onto the key frames tgt_ids each moved by tgt_pre_pose6 when given and then by its tgt_poses6
+        row.  Returns a dict (res_trans (4,4) float64, status, status_name, iterations, admm_iterations, scale, mu_source,
+        mu_target, n_source, n_target, n_source_finite, n_target_finite, primal, dual, stop, mu_exit, syncs, admm_blocks) and, in this
+        order when asked for, the last ICP iteration's matched target index (-1: none) and residual of every source point,
+        and the per-ICP-iteration log ((k, 5): ADMM iterations, primal, dual, stop, μ at exit)."""
+        def cfg():
+            return SicpConfig(float(p), float(mu), float(alpha), float(max_mu), int(max_icp), int(max_outer), float(stop))
+        return self._reloc("flb_keyframes_sicp", cfg, SicpResult(), lambda r: {
+            "res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
+            "status_name": FRICP_STATUS[r.status], "iterations": r.iterations, "admm_iterations": r.admm_iterations,
+            "scale": r.scale, "mu_source": np.array(r.mu_source[:]), "mu_target": np.array(r.mu_target[:]),
+            "n_source": r.n_source, "n_target": r.n_target, "n_source_finite": r.n_source_finite,
+            "n_target_finite": r.n_target_finite, "primal": r.primal, "dual": r.dual, "stop": r.stop, "mu_exit": r.mu_exit,
+            "syncs": r.syncs, "admm_blocks": r.admm_blocks},
+            src_points, tgt_ids, tgt_poses6, tgt_pre_pose6, src_pose6, correspondences, log, log_cap, 5)
 
     def aaicp(self, src_points, tgt_ids, tgt_poses6, tgt_pre_pose6=None, src_pose6=None, max_icp=100, stop=1e-5,
               error_overflow_threshold=0.05, correspondences=False, log=False, log_cap=4096):
@@ -1075,36 +1062,15 @@ class KeyFrameStore:
         asked for, the last pass's matched target index (-1: none) and residual of every source point, and the
         per-iteration log ((k, 6): energy, previous energy, outcome (-1 first, 1 accepted, 0 reset), α count,
         |final - final_prev|_F, smallest alphas_cond margin)."""
-        pts, stride, off_i = self._source(src_points)
-        n = len(pts)
-        ids = np.ascontiguousarray(tgt_ids, np.int32).reshape(-1)
-        p6 = np.ascontiguousarray(tgt_poses6, np.float32).reshape(-1, 6)
-        if len(p6) != len(ids):
-            raise ValueError("one pose per target key frame")
-        pre = None if tgt_pre_pose6 is None else np.ascontiguousarray(tgt_pre_pose6, np.float32).reshape(6)
-        sp = None if src_pose6 is None else np.ascontiguousarray(src_pose6, np.float32).reshape(6)
-        cfg = AaicpConfig(int(max_icp), float(stop), float(error_overflow_threshold))
-        r = AaicpResult()
-        idx = resid = lg = None
-        if correspondences:
-            idx = np.empty(max(n, 1), np.int32)
-            resid = np.empty(max(n, 1), np.float64)
-        if log:
-            lg = np.zeros((max(int(log_cap), 1), 6), np.float64)
-        _chk(lib().flb_keyframes_aaicp(self.h, _p(pts) if n else None, n, stride, off_i, _p(sp), _p(ids) if len(ids) else None, len(ids),
-                                       _p(pre), _p(p6) if len(ids) else None, C.byref(cfg), C.byref(r), _p(idx), _p(resid), _p(lg),
-                                       int(log_cap) if log else 0))
-        res = {"res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
-               "status_name": FRICP_STATUS[r.status], "iterations": r.iterations, "accepted": r.accepted, "resets": r.resets,
-               "history": r.history, "energy": r.energy, "scale": r.scale, "mu_source": np.array(r.mu_source[:]),
-               "mu_target": np.array(r.mu_target[:]), "n_source": r.n_source, "n_target": r.n_target,
-               "n_source_finite": r.n_source_finite, "n_target_finite": r.n_target_finite, "syncs": r.syncs}
-        out = (res,)
-        if correspondences:
-            out += (idx[:n].copy(), resid[:n].copy())
-        if log:
-            out += (lg[:r.log_n].copy(),)
-        return out if len(out) > 1 else res
+        def cfg():
+            return AaicpConfig(int(max_icp), float(stop), float(error_overflow_threshold))
+        return self._reloc("flb_keyframes_aaicp", cfg, AaicpResult(), lambda r: {
+            "res_trans": np.array(r.res_trans[:], np.float64).reshape(4, 4), "status": r.status,
+            "status_name": FRICP_STATUS[r.status], "iterations": r.iterations, "accepted": r.accepted, "resets": r.resets,
+            "history": r.history, "energy": r.energy, "scale": r.scale, "mu_source": np.array(r.mu_source[:]),
+            "mu_target": np.array(r.mu_target[:]), "n_source": r.n_source, "n_target": r.n_target,
+            "n_source_finite": r.n_source_finite, "n_target_finite": r.n_target_finite, "syncs": r.syncs},
+            src_points, tgt_ids, tgt_poses6, tgt_pre_pose6, src_pose6, correspondences, log, log_cap, 6)
 
 
 def make_fov(cube_len=200.0, det_range=100.0):

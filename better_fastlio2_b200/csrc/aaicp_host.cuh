@@ -284,22 +284,12 @@ extern "C" int flb_keyframes_aaicp(flb_keyframes* k, const void* src_pts, int n_
                                    const float* src_pose6, const int* tgt_ids, int n_tgt, const float* tgt_pre_pose6,
                                    const float* tgt_poses6, const flb_aaicp_config* cfg, flb_aaicp_result* out, int* out_corr_index,
                                    double* out_resid, double* out_log, int log_cap) {
-  const char* who = "flb_keyframes_aaicp";
-  if (!out) return set_err("%s: null result", who);
-  if (!cfg) return set_err("%s: null config", who);
-  if (aaicp_cfg_check(cfg, who)) return 1;
   FrSetup st;
-  if (fr_setup(k, who, src_pts, n_src, src_stride, src_off_intensity, src_pose6, tgt_ids, n_tgt, tgt_pre_pose6, tgt_poses6,
-               out_corr_index, out_resid, out_log, log_cap, 1, &st))
+  flb_aaicp_result res;
+  if (fr_open(k, "flb_keyframes_aaicp", cfg, aaicp_cfg_check, src_pts, n_src, src_stride, src_off_intensity, src_pose6, tgt_ids,
+              n_tgt, tgt_pre_pose6, tgt_poses6, out_corr_index, out_resid, out_log, log_cap, 1, out, res, st))
     return 1;
-  flb_aaicp_result res{};
-  for (int i = 0; i < 16; ++i) res.res_trans[i] = (i % 5 == 0) ? 1.0 : 0.0;
-  fr_setup_result(st, res);
-  res.syncs = st.syncs;
-  if (st.status >= 0) {
-    *out = res;
-    return 0;
-  }
+  if (st.status >= 0) return 0;
   flb_map* m = k->map;
   KfWork& kw = *m->kfw;
   IcpIndex& x = kw.index;
@@ -390,17 +380,11 @@ extern "C" int flb_keyframes_aaicp(flb_keyframes* k, const void* src_pts, int n_
   memcpy(xf.m, fin, sizeof(xf.m));
   if (icp_reduce<1>(m, x, n_s, AaEnergyOp{xf, w.x.p, w.sorted_d.p, w.pos.p, passes > 0 ? 1 : 0}, w.sums.p + FR_SUM_MED)) return 1;
   CU(cudaMemcpyAsync(w.h_sums.p + FR_SUM_MED, w.sums.p + FR_SUM_MED, sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-  if (passes > 0 && fr_outputs(m, kw, n_s, out_corr_index, out_resid)) return 1;
-  CU(cudaStreamSynchronize(m->stream));
-  res.syncs++;
+  if (fr_close(m, st, fin, passes > 0, out_corr_index, out_resid, res)) return 1;
   res.energy = w.h_sums.p[FR_SUM_MED];
   res.iterations = icp;
   res.history = (int)u.size();
   res.log_n = log_n;
-  double T12[12];
-  memcpy(T12, fin, sizeof(T12));
-  fr_res_trans(st, T12, res.res_trans);
-  res.status = FLB_FRICP_OK;
   *out = res;
   return 0;
 }

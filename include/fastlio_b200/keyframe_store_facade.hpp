@@ -268,66 +268,21 @@ class KeyFrameStore {
   template <class Cloud, class Pose, class Poses6D, class Mat>
   bool fricp(const Cloud& curCloud, const Pose& initPose, const std::vector<int>& ids, const Pose& pose_ext, const Poses6D& poses6D,
              const FricpParams& params, Mat& T, flb_fricp_result* info = nullptr) {
-    typedef typename std::remove_reference<decltype(curCloud.points[0])>::type P;
-    const int n = (int)curCloud.points.size();
-    const P* p0 = n ? &curCloud.points[0] : nullptr;
-    const int off_i = n ? (int)((const char*)&p0->intensity - (const char*)p0) : -1;
-    const float init6[6] = {initPose.x, initPose.y, initPose.z, initPose.roll, initPose.pitch, initPose.yaw};
-    const float ext6[6] = {pose_ext.x, pose_ext.y, pose_ext.z, pose_ext.roll, pose_ext.pitch, pose_ext.yaw};
-    const std::vector<float> p6 = poses6(ids, poses6D);
-    flb_fricp_result r{};
-    if (!ok(flb_keyframes_fricp(kf_, p0, n, (int)sizeof(P), off_i, init6, ids.data(), (int)ids.size(), ext6, p6.data(), &params.cfg, &r,
-                                nullptr, nullptr, nullptr, 0),
-            "fricp"))
-      return false;
-    for (int i = 0; i < 4; ++i)
-      for (int j = 0; j < 4; ++j) T(i, j) = r.res_trans[4 * i + j];
-    if (info) *info = r;
-    return true;
+    return run_reloc(flb_keyframes_fricp, "fricp", curCloud, initPose, ids, pose_ext, poses6D, params.cfg, T, info);
   }
 
   // The same registration with regMode 7 (Sparse ICP, registeration.h:143-146): the clouds of fricp(), the result into T.
   template <class Cloud, class Pose, class Poses6D, class Mat>
   bool sicp(const Cloud& curCloud, const Pose& initPose, const std::vector<int>& ids, const Pose& pose_ext, const Poses6D& poses6D,
             const SicpParams& params, Mat& T, flb_sicp_result* info = nullptr) {
-    typedef typename std::remove_reference<decltype(curCloud.points[0])>::type P;
-    const int n = (int)curCloud.points.size();
-    const P* p0 = n ? &curCloud.points[0] : nullptr;
-    const int off_i = n ? (int)((const char*)&p0->intensity - (const char*)p0) : -1;
-    const float init6[6] = {initPose.x, initPose.y, initPose.z, initPose.roll, initPose.pitch, initPose.yaw};
-    const float ext6[6] = {pose_ext.x, pose_ext.y, pose_ext.z, pose_ext.roll, pose_ext.pitch, pose_ext.yaw};
-    const std::vector<float> p6 = poses6(ids, poses6D);
-    flb_sicp_result r{};
-    if (!ok(flb_keyframes_sicp(kf_, p0, n, (int)sizeof(P), off_i, init6, ids.data(), (int)ids.size(), ext6, p6.data(), &params.cfg, &r,
-                               nullptr, nullptr, nullptr, 0),
-            "sicp"))
-      return false;
-    for (int i = 0; i < 4; ++i)
-      for (int j = 0; j < 4; ++j) T(i, j) = r.res_trans[4 * i + j];
-    if (info) *info = r;
-    return true;
+    return run_reloc(flb_keyframes_sicp, "sicp", curCloud, initPose, ids, pose_ext, poses6D, params.cfg, T, info);
   }
 
   // The same registration with regMode 1 (AA-ICP, registeration.h:86-91): the clouds of fricp(), the result into T.
   template <class Cloud, class Pose, class Poses6D, class Mat>
   bool aaicp(const Cloud& curCloud, const Pose& initPose, const std::vector<int>& ids, const Pose& pose_ext, const Poses6D& poses6D,
              const AaicpParams& params, Mat& T, flb_aaicp_result* info = nullptr) {
-    typedef typename std::remove_reference<decltype(curCloud.points[0])>::type P;
-    const int n = (int)curCloud.points.size();
-    const P* p0 = n ? &curCloud.points[0] : nullptr;
-    const int off_i = n ? (int)((const char*)&p0->intensity - (const char*)p0) : -1;
-    const float init6[6] = {initPose.x, initPose.y, initPose.z, initPose.roll, initPose.pitch, initPose.yaw};
-    const float ext6[6] = {pose_ext.x, pose_ext.y, pose_ext.z, pose_ext.roll, pose_ext.pitch, pose_ext.yaw};
-    const std::vector<float> p6 = poses6(ids, poses6D);
-    flb_aaicp_result r{};
-    if (!ok(flb_keyframes_aaicp(kf_, p0, n, (int)sizeof(P), off_i, init6, ids.data(), (int)ids.size(), ext6, p6.data(), &params.cfg, &r,
-                                nullptr, nullptr, nullptr, 0),
-            "aaicp"))
-      return false;
-    for (int i = 0; i < 4; ++i)
-      for (int j = 0; j < 4; ++j) T(i, j) = r.res_trans[4 * i + j];
-    if (info) *info = r;
-    return true;
+    return run_reloc(flb_keyframes_aaicp, "aaicp", curCloud, initPose, ids, pose_ext, poses6D, params.cfg, T, info);
   }
 
   // pcl::copyPointCloud(*surfCloudKeyFrames[k], out)
@@ -363,6 +318,29 @@ class KeyFrameStore {
       for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 4; ++c) t[j * 12 + r * 4 + c] = T[j](r, c);
     return t;
+  }
+  // fricp / sicp / aaicp through their C entry point fn: curCloud's records uploaded as they are, res_trans into T
+  template <class Cfg, class R, class Cloud, class Pose, class Poses6D, class Mat>
+  bool run_reloc(int (*fn)(flb_keyframes*, const void*, int, int, int, const float*, const int*, int, const float*, const float*,
+                           const Cfg*, R*, int*, double*, double*, int),
+                 const char* what, const Cloud& curCloud, const Pose& initPose, const std::vector<int>& ids, const Pose& pose_ext,
+                 const Poses6D& poses6D, const Cfg& cfg, Mat& T, R* info) {
+    typedef typename std::remove_reference<decltype(curCloud.points[0])>::type P;
+    const int n = (int)curCloud.points.size();
+    const P* p0 = n ? &curCloud.points[0] : nullptr;
+    const int off_i = n ? (int)((const char*)&p0->intensity - (const char*)p0) : -1;
+    const float init6[6] = {initPose.x, initPose.y, initPose.z, initPose.roll, initPose.pitch, initPose.yaw};
+    const float ext6[6] = {pose_ext.x, pose_ext.y, pose_ext.z, pose_ext.roll, pose_ext.pitch, pose_ext.yaw};
+    const std::vector<float> p6 = poses6(ids, poses6D);
+    R r{};
+    if (!ok(fn(kf_, p0, n, (int)sizeof(P), off_i, init6, ids.data(), (int)ids.size(), ext6, p6.data(), &cfg, &r, nullptr, nullptr,
+               nullptr, 0),
+            what))
+      return false;
+    for (int i = 0; i < 4; ++i)
+      for (int j = 0; j < 4; ++j) T(i, j) = r.res_trans[4 * i + j];
+    if (info) *info = r;
+    return true;
   }
   template <class Mat>
   bool run_scan_context(const std::vector<int>& ids, int kind, const std::vector<float>& t, double lidar_height, Mat& desc) {
