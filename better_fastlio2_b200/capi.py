@@ -121,6 +121,25 @@ class IcpResult(C.Structure):
                 ("n_source", C.c_int), ("n_target", C.c_int), ("n_correspondences", C.c_int), ("fitness_score", C.c_double)]
 
 
+class ImuConfig(C.Structure):
+    _fields_ = [("Lidar_T_wrt_IMU", C.c_double * 3), ("Lidar_R_wrt_IMU", C.c_double * 9), ("cov_gyr_scale", C.c_double * 3),
+                ("cov_acc_scale", C.c_double * 3), ("cov_bias_gyr", C.c_double * 3), ("cov_bias_acc", C.c_double * 3)]
+
+
+class ImuResult(C.Structure):
+    _fields_ = [("status", C.c_int), ("n_poses", C.c_int), ("n_predicts", C.c_int), ("n_down", C.c_int), ("gpu_ms", C.c_float)]
+
+
+class ImuState(C.Structure):
+    _fields_ = [("mean_acc", C.c_double * 3), ("mean_gyr", C.c_double * 3), ("cov_acc", C.c_double * 3), ("cov_gyr", C.c_double * 3),
+                ("last_lidar_end_time", C.c_double), ("angvel_last", C.c_double * 3), ("acc_s_last", C.c_double * 3),
+                ("last_imu", C.c_double * 7), ("init_iter_num", C.c_int), ("imu_need_init", C.c_int), ("b_first_frame", C.c_int),
+                ("n_poses", C.c_int)]
+
+
+IMU_EMPTY, IMU_INIT, IMU_PROPAGATED = 0, 1, 2
+
+
 class IcpBatchStats(C.Structure):
     _fields_ = [("rounds", C.c_int), ("setup_syncs", C.c_int), ("iteration_syncs", C.c_int)]
 
@@ -153,6 +172,8 @@ EXPORTS = [
     "flb_fricp_default_config", "flb_keyframes_fricp", "flb_sicp_default_config", "flb_keyframes_sicp",
     "flb_aaicp_default_config", "flb_keyframes_aaicp",
     "flb_frontend_camera_config", "flb_frontend_camera_image", "flb_frontend_points_colorize", "flb_frontend_points_to_imu",
+    "flb_imu_default_config", "flb_imu_create", "flb_imu_destroy", "flb_imu_reset", "flb_imu_process",
+    "flb_imu_download_poses", "flb_imu_info",
 ]
 
 
@@ -265,6 +286,15 @@ def lib():
         L.flb_aaicp_default_config.restype = None
         L.flb_keyframes_aaicp.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, fp, vp, C.c_int, fp, fp, C.POINTER(AaicpConfig),
                                           C.POINTER(AaicpResult), vp, dp, dp, C.c_int]
+        L.flb_imu_default_config.argtypes = [C.POINTER(ImuConfig)]
+        L.flb_imu_default_config.restype = None
+        L.flb_imu_create.argtypes = [vp, C.POINTER(ImuConfig), C.POINTER(vp)]
+        L.flb_imu_destroy.argtypes = [vp]
+        L.flb_imu_destroy.restype = None
+        L.flb_imu_reset.argtypes = [vp]
+        L.flb_imu_process.argtypes = [vp, dp, C.c_int, C.c_double, C.c_double, dp, dp, C.c_float, C.POINTER(ImuResult)]
+        L.flb_imu_download_poses.argtypes = [vp, dp, C.c_int, ip]
+        L.flb_imu_info.argtypes = [vp, C.POINTER(ImuState)]
         _lib = L
     return _lib
 
@@ -723,6 +753,71 @@ class FrontEnd:
         out = np.empty((self.cap, 4), np.float32)
         _chk(lib().flb_frontend_points_to_imu(self.h, _p(st), _p(out), self.cap, C.byref(cnt)))
         return out[:cnt.value].copy()
+
+
+def imu_config(**kw):
+    """flb_imu_config with laserMapping.cpp's defaults; keyword arguments override fields (sequences of 3 or 9 values)."""
+    c = ImuConfig()
+    lib().flb_imu_default_config(C.byref(c))
+    for k, v in kw.items():
+        arr = getattr(c, k)
+        v = np.asarray(v, np.float64).reshape(-1)
+        if len(v) != len(arr):
+            raise ValueError(f"{k} takes {len(arr)} values")
+        for i, x in enumerate(v):
+            arr[i] = float(x)
+    return c
+
+
+class Imu:
+    """ImuProcess on a front end (IMU_Processing.hpp): IMU_init on the host, the forward propagation, the undistortion
+    and the voxel filter of the front end's current raw scan on the device."""
+
+    def __init__(self, frontend, cfg=None, **kw):
+        self.frontend = frontend
+        self.h = C.c_void_p()
+        c = cfg if cfg is not None else imu_config(**kw)
+        _chk(lib().flb_imu_create(frontend.h, C.byref(c), C.byref(self.h)))
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().flb_imu_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def reset(self):
+        _chk(lib().flb_imu_reset(self.h))
+
+    def process(self, imu7, lidar_beg_time, lidar_end_time, state26, P, leaf=0.0):
+        """Process(meas, kf, feats_undistort): imu7 (n,7) = stamp, acc, gyro of meas.imu.  Returns (state26, P, result) with
+        the prior; the inputs are not modified."""
+        a = np.ascontiguousarray(np.asarray(imu7, np.float64).reshape(-1, 7))
+        x = np.array(state26, np.float64, copy=True).reshape(26)
+        Pm = np.array(P, np.float64, copy=True).reshape(23, 23)
+        r = ImuResult()
+        _chk(lib().flb_imu_process(self.h, _p(a) if len(a) else None, len(a), float(lidar_beg_time), float(lidar_end_time), _p(x),
+                                   _p(Pm), float(leaf), C.byref(r)))
+        if r.n_down >= 0:
+            self.frontend.session.n = r.n_down
+        return x, Pm, r
+
+    def poses(self):
+        n = C.c_int(0)
+        _chk(lib().flb_imu_download_poses(self.h, None, 0, C.byref(n)))
+        out = np.zeros((max(n.value, 1), 22))
+        _chk(lib().flb_imu_download_poses(self.h, _p(out), n.value, C.byref(n)))
+        return out[:n.value]
+
+    def info(self):
+        s = ImuState()
+        _chk(lib().flb_imu_info(self.h, C.byref(s)))
+        d = {k: (np.array(getattr(s, k)) if isinstance(getattr(s, k), C.Array) else getattr(s, k)) for k, _ in ImuState._fields_}
+        return d
 
 
 # Preprocess parameters (preprocess.h:8-14, laserMapping.cpp:2034-2041)

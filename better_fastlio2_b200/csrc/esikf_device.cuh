@@ -148,9 +148,9 @@ __device__ __noinline__ void so3_boxminus(const double* xq, const double* oq, do
   qmul(qc, xq, q);
   log_quat(q, r);
 }
-__device__ __noinline__ void so3_boxplus(double* xq, const double* d) {
+__device__ __noinline__ void so3_boxplus(double* xq, const double* d, double scale = 1.0) {   // x * exp(d, scale / 2)
   double q[4];
-  exp_quat(d, 0.5, q);
+  exp_quat(d, scale / 2, q);
   qmul(xq, q, xq);
 }
 __device__ __noinline__ void s2_boxminus(const double* v, const double* ov, double* r) {  // S2.hpp:144-167

@@ -1778,3 +1778,4 @@ extern "C" int flb_debug_trace_read(unsigned long long* out, long long* phases, 
 #include "sicp_host.cuh"
 #include "aaicp_host.cuh"
 #include "color_host.cuh"
+#include "imu_host.cuh"

@@ -149,6 +149,27 @@ extern "C" int flb_frontend_upload(flb_frontend* f, const void* pts, int n, int 
   return upload_records(m, m->stream, f->raw, (size_t)f->cap * (size_t)stride, pts, n, stride, off_intensity, off_curvature, f->pts, f->curv);
 }
 
+// time sort + backward compensation of the current raw scan (n_raw > 0) with the poses in f->d_poses, on the map stream.
+// end26 / np_dev null: end pose `e` and n_poses from the host; else both are read on the device and n_poses is the
+// capacity the launch reserves (see k_undistort).
+static int fe_undistort_enqueue(flb_frontend* f, int n_poses, const UndistortEnd& e, const double* end26, const int* np_dev) {
+  flb_map* m = f->ses->map;
+  cudaStream_t st = m->stream;
+  const int n = f->n_raw;
+  const int g = grid_for(n, 256, m->sm_count * 8);
+  // sort(pcl_out.points.begin(), pcl_out.points.end(), time_list)  (IMU_Processing.hpp:243) — stable here
+  VgWork& v = f->vg;
+  k_time_keys<<<g, 256, 0, st>>>(f->curv, v.keys_a.p, v.vals_a.p, n);
+  size_t tb = v.tmp.cap;
+  CU(cub::DeviceRadixSort::SortPairs(v.tmp.p, tb, (const unsigned*)v.keys_a.p, v.keys_b.p, (const int*)v.vals_a.p, f->perm, n, 0, 32, st));
+  k_undistort<<<g, 256, sizeof(double) * IMU_POSE_DOUBLES * (size_t)n_poses, st>>>(f->pts, f->curv, f->perm, n, f->d_poses, n_poses, e,
+                                                                                  f->pts_t, f->curv_t, end26, np_dev);
+  m->launches += 2 + 5;
+  CU(cudaGetLastError());
+  f->sorted = true;
+  return 0;
+}
+
 extern "C" int flb_frontend_undistort(flb_frontend* f, const double* imu_poses22, int n_poses, const double* state26_end) {
   if (!f) return set_err("null front end");
   if (!imu_poses22 || !state26_end) return set_err("flb_frontend_undistort: null argument");
@@ -163,21 +184,10 @@ extern "C" int flb_frontend_undistort(flb_frontend* f, const double* imu_poses22
   memcpy(f->h_poses, imu_poses22, sizeof(double) * IMU_POSE_DOUBLES * (size_t)n_poses);
   CU(cudaMemcpyAsync(f->d_poses, f->h_poses, sizeof(double) * IMU_POSE_DOUBLES * (size_t)n_poses, cudaMemcpyHostToDevice, st));
   CU(cudaEventRecord(f->ev_poses, st));
-  const int g = grid_for(n, 256, m->sm_count * 8);
-  // sort(pcl_out.points.begin(), pcl_out.points.end(), time_list)  (IMU_Processing.hpp:243) — stable here
-  VgWork& v = f->vg;
-  k_time_keys<<<g, 256, 0, st>>>(f->curv, v.keys_a.p, v.vals_a.p, n);
-  size_t tb = v.tmp.cap;
-  CU(cub::DeviceRadixSort::SortPairs(v.tmp.p, tb, (const unsigned*)v.keys_a.p, v.keys_b.p, (const int*)v.vals_a.p, f->perm, n, 0, 32, st));
   UndistortEnd e;
   for (int k = 0; k < 4; ++k) { e.rot[k] = state26_end[3 + k]; e.offR[k] = state26_end[7 + k]; }
   for (int k = 0; k < 3; ++k) { e.pos[k] = state26_end[k]; e.offT[k] = state26_end[11 + k]; }
-  k_undistort<<<g, 256, sizeof(double) * IMU_POSE_DOUBLES * (size_t)n_poses, st>>>(f->pts, f->curv, f->perm, n, f->d_poses, n_poses, e,
-                                                                                  f->pts_t, f->curv_t);
-  m->launches += 2 + 5;
-  CU(cudaGetLastError());
-  f->sorted = true;
-  return 0;
+  return fe_undistort_enqueue(f, n_poses, e, nullptr, nullptr);
 }
 
 extern "C" int flb_frontend_voxel_filter(flb_frontend* f, float leaf, int* n_out) {

@@ -103,10 +103,18 @@ __device__ __forceinline__ void undistort_point(float& px, float& py, float& pz,
 // the LAST segment whose head time it exceeds (what the reference's backward double sweep computes for time-sorted
 // points); points not later than IMUpose[0] stay untouched.  Quirk kept: the first sorted point is compensated again by
 // every earlier segment whose head time it exceeds (the `break` at begin() leaves the iterator on it, :382-383).
+// end26 / np_dev (both null, or both set): the end pose and the pose count come from the device (the state26 and
+// n_poses of the IMU propagation's record) instead of `e` / `np`; np is then the capacity the shared memory holds.
 __global__ void k_undistort(const float4* __restrict__ pts, const float* __restrict__ curv, const int* __restrict__ perm, int n,
                             const double* __restrict__ poses, int np, UndistortEnd e, float4* __restrict__ out,
-                            float* __restrict__ out_curv) {
+                            float* __restrict__ out_curv, const double* __restrict__ end26 = nullptr,
+                            const int* __restrict__ np_dev = nullptr) {
   extern __shared__ double sp[];
+  if (end26) {
+    np = *np_dev;
+    for (int k = 0; k < 4; ++k) { e.rot[k] = end26[3 + k]; e.offR[k] = end26[7 + k]; }
+    for (int k = 0; k < 3; ++k) { e.pos[k] = end26[k]; e.offT[k] = end26[11 + k]; }
+  }
   for (int k = threadIdx.x; k < np * IMU_POSE_DOUBLES; k += blockDim.x) sp[k] = poses[k];
   __syncthreads();
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {

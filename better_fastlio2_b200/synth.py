@@ -406,3 +406,38 @@ def driver_records(model, world, state_true, rng, with_time=True, scan_time=0.1,
     ins = np.concatenate([extra + 1, rep + 1])
     order = np.argsort(ins, kind="stable")
     return np.insert(rec, ins[order], np.concatenate([dup, rep_rec])[order])
+
+
+# ------------------------------------------------------------------------------------------------ IMU streams
+G_M_S2 = 9.81
+
+
+def imu_trajectory(t, speed=10.0, z=1.8, yaw_amp_deg=4.0):
+    """Analytic motion behind trajectory_state (scan k at t = 0.1 k): position, rotation, world acceleration and body
+    rate at time t (seconds).  Drives along +x with y = 1.5 sin(0.2 t) and yaw = amp sin(0.5 t)."""
+    amp = np.deg2rad(yaw_amp_deg)
+    pos = np.array([speed * t, 1.5 * np.sin(0.2 * t), z])
+    acc = np.array([0.0, -1.5 * 0.04 * np.sin(0.2 * t), 0.0])
+    yaw = amp * np.sin(0.5 * t)
+    R = quat_to_mat(quat_from_rotvec([0.0, 0.0, yaw]))
+    omega = np.array([0.0, 0.0, 0.5 * amp * np.cos(0.5 * t)])
+    return pos, R, acc, omega
+
+
+def imu_samples(t_beg, t_end, rate_hz, rng, gyro_bias=(0.002, -0.001, 0.003), acc_bias=(0.02, -0.01, 0.03), gyro_noise=1e-3,
+                acc_noise=1e-2, g_units=False, offset=0.0, **traj):
+    """IMU messages with stamps on the grid offset + m / rate_hz inside [t_beg, t_end): (n, 7) = stamp, acc, gyro.
+    gyro = body rate + bias + noise, acc = R^T (p'' - g) + bias + noise with g = (0, 0, -G_m_s2); g_units=True divides
+    the acceleration by G_m_s2 (drivers that report in g).  Scan k of driver_records spans [0.1 k, 0.1 k + 0.1)."""
+    m0 = int(np.ceil((t_beg - offset) * rate_hz - 1e-9))
+    m1 = int(np.ceil((t_end - offset) * rate_hz - 1e-9))
+    out = []
+    for m in range(m0, m1):
+        t = offset + m / rate_hz
+        _, R, a_w, om = imu_trajectory(t, **traj)
+        f = R.T @ (a_w - np.array([0.0, 0.0, -G_M_S2])) + np.asarray(acc_bias) + rng.normal(0, acc_noise, 3)
+        if g_units:
+            f = f / G_M_S2
+        w = om + np.asarray(gyro_bias) + rng.normal(0, gyro_noise, 3)
+        out.append(np.concatenate([[t], f, w]))
+    return np.array(out, np.float64).reshape(-1, 7)

@@ -266,8 +266,8 @@ void flb_frontend_destroy(flb_frontend* f);
  * (n * stride_bytes bytes are copied), as a std::vector<PointType> / pcl::PointCloud does. */
 int flb_frontend_upload(flb_frontend* f, const void* pts, int n, int stride_bytes, int off_intensity, int off_curvature);
 /* ImuProcess::UndistortPcl, the per-point part (IMU_Processing.hpp:243 sort by time, :334-386 backward compensation).
- * imu_poses = n_poses x 22 doubles = the IMUpose vector built by the forward propagation (:260-322, stays on the host
- * with kf.predict); state26_end = imu_state after the last predict (:329).  Result: feats_undistort in time order
+ * imu_poses = n_poses x 22 doubles = the IMUpose vector built by a host-side forward propagation (:260-322, kf.predict;
+ * flb_imu_process below runs it on the device instead); state26_end = imu_state after the last predict (:329).  Result: feats_undistort in time order
  * (ties keep upload order; the reference's std::sort leaves them unspecified). */
 int flb_frontend_undistort(flb_frontend* f, const double* imu_poses, int n_poses, const double* state26_end);
 /* downSizeFilterSurf.setInputCloud(feats_undistort); downSizeFilterSurf.filter(*feats_down_body)
@@ -639,6 +639,62 @@ int flb_keyframes_aaicp(flb_keyframes* kf, const void* src_points, int n_src, in
                         const float* src_pose6, const int* tgt_ids, int n_tgt, const float* tgt_pre_pose6, const float* tgt_poses6,
                         const flb_aaicp_config* cfg, flb_aaicp_result* out, int* out_corr_index, double* out_resid,
                         double* out_log, int log_cap);
+
+/* ------------------------------------------------------------------------------------------------ IMU propagation
+ * ImuProcess::Process (src/IMU_Processing.hpp:393-434) on a front end: IMU_init (:174-233, with the MAX_INI_COUNT logic
+ * of :405-427) on the host, the forward propagation of UndistortPcl (:241-331, kf.predict esekfom.hpp:280-384) in one
+ * device kernel that writes IMUpose and the end state where the undistortion reads them, then the undistortion and
+ * (optionally) the voxel filter of the front end's current raw scan.  DESIGN.md §10 states the contract. */
+typedef struct flb_imu flb_imu;
+
+typedef struct flb_imu_config {
+  double Lidar_T_wrt_IMU[3];  /* set_extrinsic (laserMapping.cpp:2142-2143) */
+  double Lidar_R_wrt_IMU[9];  /* row-major rotation */
+  double cov_gyr_scale[3];    /* set_gyr_cov: cov_gyr after initialisation */
+  double cov_acc_scale[3];    /* set_acc_cov: cov_acc after initialisation */
+  double cov_bias_gyr[3];     /* set_gyr_bias_cov */
+  double cov_bias_acc[3];     /* set_acc_bias_cov */
+} flb_imu_config;
+
+/* status of flb_imu_process */
+#define FLB_IMU_EMPTY 0       /* meas.imu empty: nothing done (:398-401) */
+#define FLB_IMU_INIT 1        /* IMU_init ran; state26 / P written; the scan was not touched (:405-427) */
+#define FLB_IMU_PROPAGATED 2  /* propagated and undistorted (:430) */
+
+typedef struct flb_imu_result {
+  int status;
+  int n_poses;        /* IMUpose.size() (1 + the segments that were not skipped) */
+  int n_predicts;     /* kf.predict calls: n_poses - 1 + 1 */
+  int n_down;         /* feats_down_size when leaf > 0, else -1 */
+  float gpu_ms;       /* device time of the call from the staging upload to the read-back (0 unless status 2) */
+} flb_imu_result;
+
+typedef struct flb_imu_state {  /* the persistent members of ImuProcess */
+  double mean_acc[3], mean_gyr[3], cov_acc[3], cov_gyr[3];
+  double last_lidar_end_time; /* last_lidar_end_time_ (0 before the first propagation) */
+  double angvel_last[3], acc_s_last[3];
+  double last_imu[7];         /* last_imu_: stamp, acc, gyro (zero before the first sample) */
+  int init_iter_num, imu_need_init, b_first_frame, n_poses;
+} flb_imu_state;
+
+/* laserMapping.cpp's defaults (:51, :2142-2146): gyr / acc 0.1, biases 1e-4, identity extrinsic. */
+void flb_imu_default_config(flb_imu_config* cfg);
+/* Every field must be finite; errors name the field.  The propagation uses the front end's stream and pose buffer. */
+int flb_imu_create(flb_frontend* fe, const flb_imu_config* cfg, flb_imu** out);
+void flb_imu_destroy(flb_imu* imu);
+/* ImuProcess::Reset (:90-102): b_first_frame_ is left as it is. */
+int flb_imu_reset(flb_imu* imu);
+/* p_imu->Process(Measures, kf, feats_undistort) (laserMapping.cpp:2256).  imu7 = the n_imu samples of meas.imu in order
+ * (stamp, ax, ay, az, gx, gy, gz), 0 <= n_imu <= FLB_MAX_IMU_POSES - 1; state26 / P (23x23 row-major) come in as
+ * kf.get_x() / kf.get_P() and go out as the prior.  The scan is the front end's current raw scan (flb_frontend_upload or
+ * flb_frontend_preprocess); leaf > 0 then runs the voxel filter into feats_down_body as flb_frontend_voxel_filter does.
+ * A propagation (status 2) ends in exactly one synchronisation, which returns the prior, P and the filtered count.
+ * Non-finite samples, times or state and n_imu out of range are rejected with nothing changed. */
+int flb_imu_process(flb_imu* imu, const double* imu7, int n_imu, double lidar_beg_time, double lidar_end_time, double* state26,
+                    double* P, float leaf, flb_imu_result* out);
+/* IMUpose of the last propagation (n x 22 doubles, FLB_IMU_POSE_DOUBLES layout); at most cap records, *n = its size. */
+int flb_imu_download_poses(flb_imu* imu, double* out22, int cap, int* n);
+int flb_imu_info(const flb_imu* imu, flb_imu_state* out);
 
 /* Stream access for callers that overlap work (returns a cudaStream_t as void*). */
 void* flb_session_stream(flb_session* s);

@@ -28,6 +28,15 @@ inline void pack_state26(const State& s, double* o) {
   for (int i = 0; i < 4; ++i) { o[3 + i] = s.rot.coeffs()[i]; o[7 + i] = s.offset_R_L_I.coeffs()[i]; }  // Eigen order x,y,z,w
 }
 
+// the inverse of pack_state26 (grav is MTK::S2's public `vec`)
+template <class State>
+inline void unpack_state26(const double* o, State& s) {
+  for (int i = 0; i < 3; ++i) {
+    s.pos[i] = o[i]; s.offset_T_L_I[i] = o[11 + i]; s.vel[i] = o[14 + i]; s.bg[i] = o[17 + i]; s.ba[i] = o[20 + i]; s.grav.vec[i] = o[23 + i];
+  }
+  for (int i = 0; i < 4; ++i) { s.rot.coeffs()[i] = o[3 + i]; s.offset_R_L_I.coeffs()[i] = o[7 + i]; }
+}
+
 class LioGpu {
  public:
   enum RowMode { EXACT_ROWS /* boundary B1 */, COMPRESSED_ROWS /* boundary B2 */ };
